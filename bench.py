@@ -2,6 +2,7 @@
 """bench.py -- learn_from_batch steps/sec, DQN + prioritized replay, batch 512 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo's CUDA path
+    python bench.py ... --dump-outputs DIR                          # + what the last timed step computed, as .npy
     python bench.py --impl reference [--gpus N] [--steps K] ...     # the reference's CPU path (oracle port), rank 0 only
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N    # one process per GPU, NCCL gradient all-reduce
 
@@ -17,7 +18,8 @@ TD targets -> Huber head -> backward -> global norm -> [all-reduce] -> Adam -> p
   value : steps/s with the replay resident in HBM and no per-step result read-back (device-timed, max over ranks)
   e2e   : steps/s through the public plugin API with host buffers: per step 4 new host transitions are store()d
           (num_consecutive_playing_steps = 4, dqn_agent.py:37) and the loss is read back (fetch=True)
-Inputs (59 GB ring per GPU) are far larger than the 126 MB L2, so consecutive iterations cannot hit in L2.
+Inputs (59 GB ring per GPU, within the 80 GB of an H100) are far larger than the 50 MB L2, so consecutive iterations
+cannot hit in L2.
 """
 import argparse
 import json
@@ -58,11 +60,12 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA data sheet, H100 SXM at 700 W (dense bf16); not measured
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "data-sheet"
 
 
 class ClockSampler(object):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -241,7 +244,7 @@ def run_device(args):
     lib = _lib.load()
     lib.cb200_tune(b"gemm_tc", 0 if args.no_tc else 1)
     if args.no_tc:
-        os.environ["CB200_GEMM_TILED"] = "0"      # no pre-split planes / tiled tcgen05 GEMMs either
+        os.environ["CB200_GEMM_TILED"] = "0"      # no pre-split planes / tiled tensor-core GEMMs either
     random.seed(1000 + rank)
     np.random.seed(1000 + rank)
     agent = build_device_agent(args.capacity, 100 + rank, device, args.config, frame_dedup=args.frame_dedup)
@@ -276,11 +279,13 @@ def run_device(args):
            torch.cuda.Event(enable_timing=True)) for _ in range(K)]
     orig_sample = agent.sample_batch
     step_i = [0]
+    last_batch = [None]
 
     def timed_sample():
         a, b, _ = ev[step_i[0]]
         mem.kernel_events = (a, b)        # recorded immediately around the fused sample+gather launch
-        return orig_sample()
+        last_batch[0] = orig_sample()
+        return last_batch[0]
 
     agent.sample_batch = timed_sample
     t0 = torch.cuda.Event(enable_timing=True)
@@ -298,6 +303,8 @@ def run_device(args):
     agent.sample_batch = orig_sample
     mem.kernel_events = None
     ms_total = t0.elapsed_time(t1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, agent, last_batch[0])
     launches = lib.cb200_launch_count() - launches0 + agent.graph_kernel_launches - graph_launches0
     t_load = time.perf_counter()
     while time.perf_counter() - t_load < 0.6:         # same step, same load, untimed: lets the 20 ms sampler see it
@@ -311,7 +318,7 @@ def run_device(args):
     learn_us = float(np.mean([b.elapsed_time(c) for _, b, c in ev])) * 1e3
     ms_total = parallel.max_over_ranks(ms_total, device)
 
-    # ---- per-launch timing of the dominant kernel family (the tiled tcgen05 GEMMs): one traced step lists the
+    # ---- per-launch timing of the dominant kernel family (the tiled tensor-core GEMMs): one traced step lists the
     # launches, then every distinct prepared call is timed with CUDA events on the launching stream over 10
     # back-to-back launches (the step itself has host-side bubbles between some launches, which per-launch events
     # inside the step would count as kernel time).  Operands are in the L2 state the step leaves them in.
@@ -410,7 +417,7 @@ def run_device(args):
                 "d2h_bytes_per_step": d2h, "steps": Ke,
                 "what": "per step: 4 host Transitions store()d + train(fetch=True) reading the loss back"},
         "gpu_launches": int(launches),
-        "roofline": {"kernel": "gemm_tc_tiled_kernel (multi-tap tcgen05 GEMM on TMA-fed bf16 planes; all %d launches of a "
+        "roofline": {"kernel": "gemm_tc_tiled_kernel (multi-tap wgmma GEMM on TMA-fed bf16 planes; all %d launches of a "
                                "step, conv / dense forward, data and weight gradients)" % sum(
                                    o["launches_per_step"] for o in ops),
                      "bound": "tensor", "achieved": round(tiled_tflops, 1), "peak": pk["bf16_tflops_sustained"],
@@ -420,10 +427,7 @@ def run_device(args):
                      "us_per_step": round(tl_us, 1), "share_of_step": round(tl_us / (ms_total / K * 1e3), 3),
                      "share_of_step_note": "sum of the launches' stand-alone durations / step time; inside the step "
                                            "the target forward, the weight gradients and the optimizer run on side "
-                                           "streams beside the main chain, so the launches overlap.  Serialised "
-                                           "(profiles/launches_r2k_one_step.txt, ncu, one launch at a time, cold "
-                                           "caches): the same launches incl. their split-reduce passes are 545 of "
-                                           "680 us = 0.80 of the step",
+                                           "streams beside the main chain, so the launches overlap",
                      "frac_over_whole_step": round(tl_issued / (ms_total / K * 1e-3) / 1e12
                                                    / pk["bf16_tflops_sustained"], 4),
                      "issued_flops_per_step": tl_issued, "algorithmic_flops_per_step": tl_useful, "fp32_equivalent_tflops": round(tl_useful / tl_us / 1e6, 1)
@@ -431,9 +435,7 @@ def run_device(args):
                      "what": "achieved = bf16 tensor-core FLOPs issued (3xBF16 split: 6 products per fp32 MAC, 3 for "
                              "the exact uint8 operand) / CUDA-event time of the launches (each prepared call timed over "
                              "10 back-to-back launches incl. its split-reduce pass, weighted by launches per step)",
-                     "traffic": TRAFFIC_NCU.get("gemm_tc_tiled"),
-                     "traffic_note": "dram bytes summed over the launches of one step, from the committed ncu --set full "
-                                     "capture under profiles/ (cold caches), not this run", "ops": ops},
+                     "ops": ops},
         "roofline_gather": {"kernel": ("sample_gather_s2d_kernel (fused sum-tree descent + IS weights + TMA bulk-copy gather + "
                                        "uint8 -> bf16 space-to-depth operand plane of conv1: replaces the staged uint8 "
                                        "copy and the two conversion passes over it)") if agent.s2d is not None else
@@ -447,12 +449,9 @@ def run_device(args):
                                               ("; frame-deduplicated replay: 18.1 MB of distinct frames read"
                                                if mem.ring.stack_cols else ""),
                      "bytes_moved": moved,
-                     "frac_bytes_moved": round(moved / gather_us / 1e3 / pk["hbm_gbs"], 4),
-                     "traffic": TRAFFIC_NCU.get("sample_gather_s2d" if agent.s2d is not None else "per_sample_gather"),
-                     "traffic_note": "dram bytes from the committed ncu --set full capture under profiles/, not this run",
-                     "frac_of_8TBps": round(gather_gbs / 8000.0, 4)},
+                     "frac_bytes_moved": round(moved / gather_us / 1e3 / pk["hbm_gbs"], 4)},
         "roofline_learn": {"kernels": ("fp32 FFMA gather-GEMMs" if args.no_tc else
-                                       "tcgen05 gather-GEMMs (3xBF16 split, 6 MMAs per product, fp32 TMEM accumulators)")
+                                       "wgmma gather-GEMMs (3xBF16 split, 6 MMAs per product, fp32 accumulators)")
                            + " (conv/dense fwd+bwd) + element-wise",
                            "bound": "tensor", "achieved": round(gemm_tflops, 2), "peak": pk["bf16_tflops_sustained"],
                            "unit": "TFLOP/s", "frac": round(gemm_tflops / pk["bf16_tflops_sustained"], 5),
@@ -469,12 +468,35 @@ def run_device(args):
     sys.stdout.flush()
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed ncu --set full capture (profiles/)
-# (gemm_tc_tiled: sum over the 15 launches of one step, profiles/ncu_tiled_gemm_r1p_summary.txt -- cold caches under ncu)
-# dram__bytes_read.sum + dram__bytes_write.sum per launch (per step for the GEMM family: 16 launches), cold caches:
-# profiles/ncu_step_r2f_summary.txt (sample_gather_s2d: 30.4 MB read + 4.9 MB written -- the bf16 planes stay in L2),
-# profiles/ncu_tiled_r2f_summary.txt, profiles/ncu_per_sample_gather_r1b_summary.txt
-TRAFFIC_NCU = {"per_sample_gather": 30270000, "sample_gather_s2d": 35286016, "gemm_tc_tiled": 473743616}
+DUMP_TREE_NODES = 1 << 21          # 16.8 MB of fp64 (the whole tree of a 2^20-slot replay)
+
+
+def dump_outputs(out_dir, agent, batch):
+    """What the last timed step handed back or left behind, as DIR/<name>.npy (float32 / float64, at most ~47 MB): the
+    loss and TD errors of the head, the sampled indices and importance weights, the updated online parameters and the
+    PER sum tree after the priority update -- whole up to DUMP_TREE_NODES nodes, above that a fixed seeded sample of
+    DUMP_TREE_NODES of them (their positions in per_sum_tree_nodes.npy).  Inputs are seeded, so two builds can be
+    compared output for output."""
+    import torch
+    agent._join_optimizer()
+    agent._side_upd.join()
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    out = {"loss": agent.loss_dev.reshape(-1).double(), "td_errors": agent.td_err.double(),
+           "sample_indices": batch.info("idx").double(), "sample_weights": batch.column("weight32").float(),
+           "per_sum_tree": agent.memory.sum_tree.double()}
+    tree = out["per_sum_tree"]
+    if tree.numel() > DUMP_TREE_NODES:
+        nodes = np.sort(np.random.RandomState(0).choice(tree.numel(), DUMP_TREE_NODES, replace=False))
+        out["per_sum_tree"] = tree[torch.from_numpy(nodes).to(tree.device)]
+        out["per_sum_tree_nodes"] = nodes.astype(np.float64)
+    for name, v in agent.net_def.store.export_named().items():
+        out["param_" + name.replace("/", "_").replace(":", "_")] = np.asarray(v, dtype=np.float32)
+    for name, v in out.items():
+        arr = v.cpu().numpy() if hasattr(v, "cpu") else v
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
+
+
 
 
 # =====================================================================================================================
@@ -613,17 +635,23 @@ def main():
     ap.add_argument("--frame-dedup", type=int, default=0, choices=[0, 1],
                     help="1: frame-deduplicated replay -- every 84x84 frame stored once (9.3 GB instead of 59.2 GB for "
                          "2^20 transitions, 41 KB instead of 238 KB over PCIe per step), stacks assembled by the "
-                         "gather (measured 3 %% slower per step: profiles/README.md); 0 (default): stacked states "
+                         "gather; 0 (default): stacked states "
                          "verbatim")
-    ap.add_argument("--no-tc", action="store_true", help="fp32 FFMA GEMMs instead of the tcgen05 3xBF16 path")
+    ap.add_argument("--no-tc", action="store_true", help="fp32 FFMA GEMMs instead of the tensor-core 3xBF16 path")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="dqn / dueling: after the timed steps write what the last one computed to DIR/<name>.npy")
     ap.add_argument("--config", default="dqn", choices=["dqn", "dueling", "cartpole", "ppo", "sac", "td3"],
                     help="dqn: BASELINE config 2 (Atari DQN + PER, the headline metric, default); dueling: config 5 "
                          "(dueling DDQN + PER, no middleware, clip-norm 10); cartpole / ppo / sac / td3: configs 1, 3, 4 "
                          "(bench_configs.py)")
     args = ap.parse_args()
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs needs at least one timed step (--steps >= 1)")
     if args.impl == "reference":
         run_reference(args)
     elif args.config in ("cartpole", "ppo", "sac", "td3"):
+        if args.dump_outputs:
+            ap.error("--dump-outputs covers the dqn and dueling configs")
         import bench_configs
         bench_configs.run(args, ClockSampler)
         _finish()

@@ -7,7 +7,7 @@ import ctypes
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# CB200_LIB_PATH: load another build of the same library (the -DCB200_TC_PROF instrumented one of tools/tc_phase_probe.py)
+# CB200_LIB_PATH: load another build of the same library (an A/B build, for instance)
 LIB_PATH = os.environ.get("CB200_LIB_PATH") or os.path.join(_HERE, "lib", "libcoach_b200.so")
 
 c_void_p = ctypes.c_void_p
@@ -177,10 +177,11 @@ def load():
         fn.argtypes = argtypes
     if lib.cb200_abi_version() != 1:
         raise ImportError("coach_b200: ABI version mismatch between _lib.py and libcoach_b200.so")
-    # CB200_TUNE_<KEY>=<int>: runtime knobs of the library (cb200_tune), e.g. CB200_TUNE_GEMM_PERSISTENT=0 for A/B runs
+    # CB200_TUNE_<KEY>=<int>: runtime knobs of the library (cb200_tune), e.g. CB200_TUNE_GEMM_TC=0 for A/B runs
     for k, v in os.environ.items():
         if k.startswith("CB200_TUNE_"):
-            lib.cb200_tune(k[len("CB200_TUNE_"):].lower().encode(), int(v))
+            if lib.cb200_tune(k[len("CB200_TUNE_"):].lower().encode(), int(v)) != 0:
+                raise ValueError("%s: %s" % (k, lib.cb200_last_error().decode("utf-8", "replace")))
     _lib = lib
     return lib
 

@@ -600,8 +600,8 @@ class DQNAgent(object):
         single = not parallel.is_distributed()                    # no all-reduce between backward and optimizer
         # several ranks, no global-norm clipping (which needs the complete local gradient first), plain Q head: the
         # all-reduce of the dense layers' gradients can run under the conv backward pass (CB200_DQN_OVERLAP_ALLREDUCE=1).
-        # Bit-identical (tools/check_allreduce_overlap.py) but measured 1 % SLOWER at 2 and 4 GPUs (profiles/README.md):
-        # the 6.75 MB all-reduce over NVSwitch is shorter than the two extra copies and launches, so it is opt-in.
+        # Bit-identical (tools/check_allreduce_overlap.py); opt-in because the 6.75 MB all-reduce over NVSwitch is short
+        # against the two extra copies and launches it needs.
         clip = net.params.clip_gradients
         overlap = (not single) and not (clip is not None and clip != 0) and not self.net_def.dueling and \
             bool(_lib.tune_default("dqn_overlap_allreduce", 0))
@@ -641,8 +641,8 @@ class DQNAgent(object):
             self._overlapped_allreduce_end(*pending)
         elif graph and self._opt_on_stream:
             if not single:
-                # (the all-reduce stays on the main stream: issued from the optimizer's stream, beside the next sample +
-                # gather, a 2-GPU step measured 0.86 ms against 0.63 ms -- profiles/README.md r2k)
+                # (the all-reduce stays on the main stream rather than being issued from the optimizer's stream, beside
+                # the next sample + gather)
                 torch.distributed.all_reduce(net.store.grad, op=torch.distributed.ReduceOp.SUM)
             with self._side_opt:                                  # ordered after the backward graph; joined lazily
                 self._graph_c[0].replay()

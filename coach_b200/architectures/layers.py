@@ -7,7 +7,7 @@ conv kernels HWIO (= a row-major [KH*KW*Cin, N] matrix), dense kernels [in, out]
 
 Two execution forms, chosen per layer when it is prepared.  With operand planes (``planes=tiled.PlaneCtx``, batch a
 multiple of 32, channel counts the tensor-core kernel supports) forward, weight gradient and data gradient are
-multi-tap tcgen05 GEMMs on pre-split bf16 operands (``architectures/tiled.py``, cb200_gemm_tiled); the uint8 first
+multi-tap wgmma GEMMs on pre-split bf16 operands (``architectures/tiled.py``, cb200_gemm_tiled); the uint8 first
 convolution runs on the space-to-depth view of the frames (``_prepare_s2d``).  Otherwise -- small batches, odd shapes,
 the skinny Q head -- the gather-GEMM below.
 
@@ -140,10 +140,11 @@ class GemmOp(object):
         _lib.check(self.lib.cb200_gemm(ctypes.byref(self.desc), _lib.current_stream()))
 
 
-def pick_splits(tiles, reduction, sm=148, min_chunk=128):
+def pick_splits(tiles, reduction, sm=132, min_chunk=128):
     """Split the reduction so that the grid has about two CTAs per SM, never below `min_chunk` per split."""
-    # the tensor-core path accumulates in TMEM with truncation: never reduce more than TC_MAX_R terms in one launch,
-    # the partial sums are then added in fp32 round-to-nearest by the split-reduce kernel (csrc/nn_gemm_tc.cuh)
+    # the tensor-core path never reduces more than TC_MAX_R terms in one launch (the error of its fp32 accumulation
+    # grows with the accumulation count); the partial sums are then added in fp32 round-to-nearest by the
+    # split-reduce kernel (csrc/nn_gemm_tc.cuh)
     need = (reduction + TC_MAX_R - 1) // TC_MAX_R
     if tiles >= sm:          # one full wave already: the extra reduction pass would cost more than it saves
         return int(max(1, need))
@@ -160,6 +161,10 @@ def _tiles(M, N, fast=True):
     if M <= 64:
         return ((M + 31) // 32) * ((N + 31) // 32)
     if fast and N % 4 == 0:
+        if N % 16 == 0:
+            # tensor-core kernel (nn_gemm_tc.cuh): 128 x 32 or 128 x 64 tiles -- one warpgroup holds the accumulators
+            bn = 32 if N <= 32 else 64
+            return ((M + 127) // 128) * ((N + bn - 1) // bn)
         if N <= 32:
             return ((M + 255) // 256) * ((N + 31) // 32)
         if N <= 64:

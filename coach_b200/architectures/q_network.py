@@ -111,7 +111,7 @@ class QNetworkInstance(object):
         are per tower; the data gradient into the conv map is ONE multi-tap GEMM over both towers: their
         pre-activation gradients are the two "pixels" of one [2B, 512] plane matrix, the per-pixel transposed kernels
         of both towers one weight stack, and every conv pixel's tap list has one entry per tower -- so the sum
-        dV W_v^T + dA W_a^T is accumulated in TMEM instead of by a second, accumulating pass."""
+        dV W_v^T + dA W_a^T is accumulated in the tensor-core accumulators instead of by a second, accumulating pass."""
         net, dev = self.net, self.net.device
         xp = self.trunk.act_planes[-1]
         npix, C = xp.npix, xp.cols

@@ -29,7 +29,7 @@ def _dev_i32(a, device):
 
 def b_interleaved(n):
     """B operands of the N <= 64 tile width (cb200_gemm_tiled: bn = 32 / 64) use row-group interleaved planes: one
-    TMA box then delivers [b1 | b2 | b3] as ONE operand and the product set is three wide MMAs instead of six"""
+    TMA box then delivers [b1 | b2 | b3] as ONE operand (csrc/nn_gemm_tiled.cuh, kCat)"""
     return bool(_lib.tune_default("gemm_cat", 1)) and (n <= 64 or n % 128 != 0)
 
 
@@ -174,8 +174,7 @@ class ThetaPlanes(object):
         if len(self.derived) > 1 and self.theta.is_cuda and _lib.tune_default("refresh_streams", 0):
             # the derived kernels (weight permutes) and the plane split are independent readers of theta: two side
             # streams next to the caller's (parallel branches when the caller is being captured into a CUDA graph).
-            # Measured (profiles/README.md, r2h): 0.621 ms per DQN step against 0.608 ms without -- the fork / join
-            # costs more than the five small kernels gain from running side by side -- hence opt-in.
+            # Opt-in: the fork / join can cost more than the five small kernels gain from running side by side.
             from coach_b200.architectures.layers import SideStream
             if getattr(self, "_sides", None) is None:
                 self._sides = (SideStream(self.theta.device), SideStream(self.theta.device))
@@ -207,12 +206,11 @@ TILED_MAX_CHUNKS = int(os.environ.get("CB200_TILED_MAX_CHUNKS", "20"))
 SPLIT_WAVES = int(os.environ.get("CB200_SPLIT_WAVES", "2"))     # CTAs per SM a split-reduction launch aims for
 
 
-def pick_splits_tiled(tiles, total_chunks, sm=148):
-    """reduction slices of a tiled GEMM: at most TILED_MAX_CHUNKS chunks (40 accumulating MMAs) per slice -- the TMEM
-    accumulator adds with truncation, a bias that grows linearly with the accumulation count (csrc/nn_gemm_tc.cuh;
-    measured in tests/test_learn_gpu.py: 18 chunks keep every gradient of the B = 512 step within 1e-5, the 32 chunks
-    the kernel would accept put the conv1 gradient of the dueling network at 3e-5) -- and more slices when the tile
-    count alone does not fill the machine"""
+def pick_splits_tiled(tiles, total_chunks, sm=132):
+    """reduction slices of a tiled GEMM: at most TILED_MAX_CHUNKS chunks (40 accumulating k16 steps) per slice -- the
+    error of the tensor-core fp32 accumulation grows with the accumulation count (tests/test_learn_gpu.py holds every
+    gradient of the B = 512 step within 1e-5) -- and more slices when the tile count alone does not fill the
+    machine (132 SMs on an H100 SXM)"""
     need = (total_chunks + TILED_MAX_CHUNKS - 1) // TILED_MAX_CHUNKS
     if tiles >= sm:
         return int(max(1, need))

@@ -1,4 +1,4 @@
-"""Builds coach_b200/lib/libcoach_b200.so (hand-written CUDA for sm_100a) with nvcc.  No torch headers involved:
+"""Builds coach_b200/lib/libcoach_b200.so (hand-written CUDA for sm_90a) with nvcc.  No torch headers involved:
 the library is a plain C-ABI shared object (include/coach_b200.h) bound from Python with ctypes.
 
     python -m coach_b200.build            # build if sources are newer than the library
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libcoach_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",   # B200 only; no PTX fallback for other architectures
+    "-gencode", "arch=compute_90a,code=sm_90a",     # H100 only; no PTX fallback for other architectures
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--threads", "0",
@@ -47,7 +47,7 @@ def build(force=False, verbose=False):
     if not force and not needs_build():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
-    extra = os.environ.get("CB200_EXTRA_NVCC_FLAGS", "").split()      # e.g. -DCB200_TC_PROF (tools/tc_phase_probe.py)
+    extra = os.environ.get("CB200_EXTRA_NVCC_FLAGS", "").split()
     cmd = [nvcc_path()] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + \
         ["-shared", "-o", LIB_PATH + ".tmp"] + sources()
     res = subprocess.run(cmd, capture_output=True, text=True)

@@ -2,7 +2,7 @@
 
   Transition   <- core_types.py:195-310   (same constructor, same "not filled" exceptions, same __copy__)
   Batch        <- core_types.py:405-649   (host AoS->SoA view over a list of Transitions; kept for API parity)
-  DeviceBatch  -- the B200-native counterpart of Batch: the same accessors (states / next_states / actions / rewards /
+  DeviceBatch  -- the device-resident counterpart of Batch: the same accessors (states / next_states / actions / rewards /
                   game_overs / info / size / slice) but every column is a CUDA tensor that the replay's gather kernel
                   has already staged in HBM.  ``Agent.train`` in the reference forces List[Transition] through
                   ``pre_network_filter`` and ``Batch()`` (agents/agent.py:726-741); device agents call

@@ -1,4 +1,4 @@
-// coach_b200/csrc/common.cuh -- shared helpers for the sm_100a kernels behind include/coach_b200.h
+// coach_b200/csrc/common.cuh -- shared helpers for the sm_90a kernels behind include/coach_b200.h
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -28,10 +28,10 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
     if (cached[dev] == 0) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
         cached[dev] = n;
     }
     return cached[dev];
@@ -57,6 +57,10 @@ int64_t cb200_launch_count(void) { return cb200::g_launches.load(std::memory_ord
 
 int cb200_tune(const char* key, int value) {
     if (!key) return CB200_ERR_INVALID_ARGUMENT;
+    if (strcmp(key, "gemm_persistent") == 0) {
+        cb200::set_error("cb200_tune: \"gemm_persistent\" was removed (the persistent tiled-GEMM schedule no longer exists)");
+        return CB200_ERR_INVALID_ARGUMENT;
+    }
     std::lock_guard<std::mutex> g(cb200::g_tune_mutex);
     cb200::g_tune[key] = value;
     return CB200_OK;

@@ -1,6 +1,6 @@
 // coach_b200/csrc/nn.cu -- C-ABI entry points of the dense contractions of the learn step (see nn_gemm.cuh).
 #include "nn_gemm_skinny.cuh"
-#include "nn_gemm_tiled_persist.cuh"
+#include "nn_gemm_tiled.cuh"
 
 namespace cb200 {
 namespace gemm {
@@ -249,29 +249,6 @@ __global__ void __launch_bounds__(256) u8_s2d_planes_kernel(const uint8_t* __res
     }
 }
 
-template <int BN, bool kT, int NA, bool kCat = false>
-static int launch_tiled_persist(const CUtensorMap& tmA, const CUtensorMap& tmB, const TiledParams& tp,
-                                const EpiParams& ep, int M, int gx, int splits, cudaStream_t st) {
-    constexpr size_t smem = PersistCfg<BN, NA>::kSmemBytes;
-    static bool configured = false;
-    if (!configured) {
-        if (cudaFuncSetAttribute(gemm_tc_tiled_persist_kernel<BN, kT, NA, kCat>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)smem) != cudaSuccess)
-            return -1;
-        configured = true;
-    }
-    UnitGrid ug{gx, (tp.n + BN - 1) / BN, splits};
-    const int units = ug.gx * ug.gy * ug.gz;
-    const int grid = units < sm_count() ? units : sm_count();
-    gemm_tc_tiled_persist_kernel<BN, kT, NA, kCat><<<grid, kPsThreads, smem, st>>>(tmA, tmB, tp, ep, M, ug);
-    count_launch();
-    if (splits > 1) {
-        launch_split_reduce(ep, M, tp.n, st);
-        count_launch();
-    }
-    return 0;
-}
-
 // ---- small helpers -------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) colsum_stage1(const float* __restrict__ x, int64_t rows, int64_t cols,
                                                      float* __restrict__ part, int nslab) {
@@ -410,8 +387,8 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
     const bool fast = d->a_vec4 && d->n % 4 == 0 && d->ldb % 4 == 0 && d->a_cols % 4 == 0 &&
                       (reinterpret_cast<uintptr_t>(d->b) & 15) == 0 && M > 64;
     CB200_CHECK_ARG(!ones || fast, "a_ones_col needs the vectorised or the skinny path");
-    // tensor-core path (tcgen05): operands split into 3 x bf16, fp32 accumulation in TMEM; the reduction length per
-    // launch is capped (split-R) because the TMEM accumulator truncates -- see nn_gemm_tc.cuh
+    // tensor-core path (wgmma): operands split into 3 x bf16, fp32 accumulation; the reduction length per launch is
+    // capped (split-R) -- see nn_gemm_tc.cuh
     const bool tc = fast && d->n % 16 == 0 && d->n >= 16 && tune_get("gemm_tc", 1, 0, 1) != 0 && d->ldc % 4 == 0 &&
                     ((reinterpret_cast<uintptr_t>(d->c) | reinterpret_cast<uintptr_t>(d->mask_y) |
                       reinterpret_cast<uintptr_t>(d->bias)) & 15) == 0 &&
@@ -425,11 +402,11 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
               : gemm::launch_tc<BN_, false, true>(*d, M, R, splits, r_per_split, st))                         \
         : (tr ? gemm::launch_tc<BN_, true, false>(*d, M, R, splits, r_per_split, st)                          \
               : gemm::launch_tc<BN_, false, false>(*d, M, R, splits, r_per_split, st)))
+        // one warpgroup holds the accumulators of a 128 x BN tile: BN <= 64
         if (d->n <= 32) rc = CB200_TC(32);
-        else if (d->n <= 64) rc = CB200_TC(64);
-        else rc = CB200_TC(128);
+        else rc = CB200_TC(64);
 #undef CB200_TC
-        CB200_CHECK_ARG(rc == 0, "could not configure shared memory for the tcgen05 kernel");
+        CB200_CHECK_ARG(rc == 0, "could not configure shared memory for the tensor-core kernel");
         CB200_CHECK_LAUNCH();
         return CB200_OK;
     }
@@ -461,18 +438,6 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }
-
-#ifdef CB200_TC_PROF
-int cb200_tc_prof_read(unsigned long long* out16, int reset) {
-    cudaDeviceSynchronize();
-    cudaMemcpyFromSymbol(out16, gemm::g_tc_prof, sizeof(unsigned long long) * 16);
-    if (reset) {
-        unsigned long long z[16] = {0};
-        cudaMemcpyToSymbol(gemm::g_tc_prof, z, sizeof(z));
-    }
-    return CB200_OK;
-}
-#endif
 
 int cb200_gemm_tiled(const cb200_tgemm_desc* d, void* stream) {
     CB200_CHECK_ARG(d != nullptr, "null descriptor");
@@ -595,7 +560,7 @@ int cb200_gemm_tiled(const cb200_tgemm_desc* d, void* stream) {
     int splits = d->splits > 1 ? d->splits : 1;
     int cps = (total + splits - 1) / splits;
     splits = (total + cps - 1) / cps;
-    // the TMEM accumulators add with truncation: at most 64 accumulating MMAs (32 chunks) per launch slice
+    // at most 32 reduction chunks (64 accumulating k16 steps) per launch slice; slices are summed in fp32
     CB200_CHECK_ARG(cps <= 32, "too few splits: more than 32 reduction chunks (1024 terms) per slice");
     CB200_CHECK_ARG(splits == 1 || d->workspace, "split reduction needs a workspace");
     tp.chunks_per_split = cps;
@@ -615,34 +580,13 @@ int cb200_gemm_tiled(const cb200_tgemm_desc* d, void* stream) {
 #define CB200_TLC(BN_) \
     (na == 1 ? gemm::launch_tiled<BN_, false, 1, true>(maps, tp, ep, M, gx, splits, st) \
              : gemm::launch_tiled<BN_, false, 3, true>(maps, tp, ep, M, gx, splits, st))
-#define CB200_TPC(BN_) \
-    (na == 1 ? gemm::launch_tiled_persist<BN_, false, 1, true>(maps[0], maps[1], tp, ep, M, gx, splits, st) \
-             : gemm::launch_tiled_persist<BN_, false, 3, true>(maps[0], maps[1], tp, ep, M, gx, splits, st))
-#define CB200_TP(BN_)                                                                                            \
-    (na == 1 ? (d->mode ? gemm::launch_tiled_persist<BN_, true, 1>(maps[0], maps[1], tp, ep, M, gx, splits, st)   \
-                        : gemm::launch_tiled_persist<BN_, false, 1>(maps[0], maps[1], tp, ep, M, gx, splits, st)) \
-             : (d->mode ? gemm::launch_tiled_persist<BN_, true, 3>(maps[0], maps[1], tp, ep, M, gx, splits, st)   \
-                        : gemm::launch_tiled_persist<BN_, false, 3>(maps[0], maps[1], tp, ep, M, gx, splits, st)))
-    // persistent schedule (epilogue of unit i under the main loop of unit i+1) unless the bias row would need more
-    // than the 512 TMEM columns for two accumulator sets
-    // (measured, profiles/README.md: on the step's shapes the persistent schedule is not faster yet -- one producer warp
-    // and one MMA thread per SM instead of two of each -- so it is opt-in: cb200_tune("gemm_persistent", 1))
-    const bool persist = tune_get("gemm_persistent", 0, 0, 1) != 0 && !(tp.bias_row && bn == 128);
-    if (cat) {
-        if (persist) rc = bn == 32 ? CB200_TPC(32) : CB200_TPC(64);
-        else rc = bn == 32 ? CB200_TLC(32) : CB200_TLC(64);
-    } else if (persist) {
-        if (bn == 32) rc = CB200_TP(32);
-        else if (bn == 64) rc = CB200_TP(64);
-        else rc = CB200_TP(128);
-    } else if (bn == 32) rc = CB200_TL(32);
+    if (cat) rc = bn == 32 ? CB200_TLC(32) : CB200_TLC(64);
+    else if (bn == 32) rc = CB200_TL(32);
     else if (bn == 64) rc = CB200_TL(64);
     else rc = CB200_TL(128);
-#undef CB200_TP
 #undef CB200_TL
 #undef CB200_TLC
-#undef CB200_TPC
-    CB200_CHECK_ARG(rc == 0, "could not configure shared memory for the tiled tcgen05 kernel");
+    CB200_CHECK_ARG(rc == 0, "could not configure shared memory for the tiled tensor-core kernel");
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

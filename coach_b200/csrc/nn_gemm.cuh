@@ -195,7 +195,7 @@ __device__ __forceinline__ float mask_from_planes(const uint16_t* p, int64_t str
 
 // Plane format.  A logical [rows, cols] matrix (both multiples of 8) is stored as 8x8 "core matrices" of 128 contiguous
 // bytes, core (r / 8, c / 8) at ((r / 8) * (cols / 8) + c / 8) * 64 elements, element (r % 8, c % 8) inside it
-// row-major.  This is exactly the unit the tcgen05 shared-memory descriptors address without swizzling (K-major A with
+// row-major.  This is exactly the unit the wgmma shared-memory descriptors address without swizzling (K-major A with
 // M = rows, K = cols; MN-major A^T / B with K = rows, MN = cols all read the same 128 bytes), so any operand tile is a
 // handful of contiguous runs of cores that a 1-D bulk copy (TMA) moves without touching a register.
 // Activations / gradients use rows = pixel * batch + b (pixel-major, batch-inner), cols = channels: the im2col tile of
@@ -205,8 +205,8 @@ __device__ __forceinline__ size_t tiled_elem(size_t prow, int col, int pcols) {
 }
 // "Row-group interleaved" planes (B operands of the N <= 64 forward / data-gradient GEMMs): the three planes of one
 // 8-row group sit next to each other -- (row group | plane | column core | 64) -- so that ONE TMA box delivers a
-// [k-group][plane][column core] tile, i.e. a single MN-major operand [32 k, 3 * n] = [b1 | b2 | b3] whose products with
-// one A plane are issued as one tcgen05.mma of triple width (nn_gemm_tiled.cuh, kCat).  Plane stride argument -1.
+// [k-group][plane][column core] tile, i.e. a single MN-major operand [32 k, 3 * n] = [b1 | b2 | b3] fetched with one
+// box instead of three (nn_gemm_tiled.cuh, kCat).  Plane stride argument -1.
 __device__ __forceinline__ size_t tiled_elem_il(size_t prow, int col, int pcols, int plane) {
     return (((prow >> 3) * 3 + (size_t)plane) * (size_t)(pcols >> 3) + (size_t)(col >> 3)) * 64 + (prow & 7) * 8 + (col & 7);
 }

@@ -1,21 +1,19 @@
-// coach_b200/csrc/nn_gemm_tc.cuh -- the gather-GEMM on the 5th-generation tensor cores (tcgen05 + TMEM).
+// coach_b200/csrc/nn_gemm_tc.cuh -- the gather-GEMM on the Hopper tensor cores (wgmma, fp32 register accumulators).
 //
 // Same contraction / tables / epilogue as nn_gemm_fast.cuh, computed as a 3-way BF16 operand split with fp32
-// accumulation in tensor memory:
+// accumulation:
 //     x = x1 + x2 + x3 (bf16 each, exact: truncation split);   A*B ~= a1 b1 + [a1 b2 + a2 b1 + a2 b2 + a1 b3 + a3 b1]
-// Two TMEM accumulators per output tile: MAIN collects a1*b1, CORR collects the five correction products.  Measured
-// on B200 (tools/tc_probe.cu, profiles/tc_probe_r1.jsonl): the TMEM accumulator adds with truncation, so the error
-// grows with the number of accumulating MMAs (2e-5 of the output scale at K = 3136 with one accumulator).  Keeping the
-// small products in their own accumulator makes their truncation error relative to a 2^-8 smaller magnitude, and the
-// host caps the reduction length per launch (split-R, summed afterwards in fp32 round-to-nearest by
-// split_reduce_kernel), which bounds MAIN to <= 64 accumulations  =>  ~1e-6 of the output scale, i.e. fp32-level.
+// Two accumulators per output tile: MAIN collects a1*b1, CORR collects the five correction products, so the
+// truncation error of the small products stays relative to their 2^-8 smaller magnitude.  The host caps the reduction
+// length per launch (split-R, summed afterwards in fp32 round-to-nearest by split_reduce_kernel), which bounds MAIN to
+// <= 64 accumulating k16 steps.
 //
 // uint8 A operands (the Atari frames of conv1, forward and weight gradient) take the EXACT path when the caller
 // declares a_u8_div (lut[v] == v / a_u8_div): the raw integers 0..255 are exact bf16 values, so A needs ONE plane and
 // the product three MMAs (a b1 + [a b2 + a b3]); the 1 / a_u8_div scale is applied once to the accumulated sum.
 //
-// Operands are staged BY THE THREADS into the canonical no-swizzle UMMA shared-memory layouts (8 x 16-byte core
-// matrices; cute/atom/mma_traits_sm100.hpp make_umma_desc): the A operand needs table-driven gather addressing,
+// Operands are staged BY THE THREADS into the canonical no-swizzle wgmma shared-memory layouts (8 x 16-byte core
+// matrices): the A operand needs table-driven gather addressing,
 // uint8 conversion and the bf16 split, none of which TMA can do.  A is K-major when the reduction index is
 // contiguous in memory (forward / data gradients) and MN-major for the weight gradients (A^T); B [R, N] row-major is
 // always MN-major.  Within a warp the 8 lanes of a quarter-warp always write the 8 rows (16 B each) of ONE core
@@ -32,9 +30,10 @@
 // work).  The register-staged kernel below remains for uint8 sources (exact path), LUT sources and plane-less fp32
 // operands; it accepts B planes too (conv1: weights / dY), which removes the B-side split.
 //
-// CTA = 128 threads = one 128 x BN output tile.  Two shared-memory stages: while the tensor core works on chunk c
-// (asynchronously, tracked by tcgen05.commit -> mbarrier), all threads convert chunk c+1.  Thread t owns output row t
-// in the epilogue (TMEM lane t): tcgen05.ld -> bias / activation / activation-derivative mask -> global.
+// CTA = 128 threads = one warpgroup = one 128 x BN output tile (BN <= 64: the accumulators of both 64-row halves live
+// in its registers).  Two shared-memory stages: while the tensor core works on chunk c (asynchronously, one wgmma
+// commit group per chunk), all threads convert chunk c+1.  The accumulators are then staged through shared memory and
+// thread t writes output row t in the epilogue: bias / activation / activation-derivative mask -> global.
 #pragma once
 #include <cuda_bf16.h>
 
@@ -48,41 +47,71 @@ constexpr int kTcBK = 32;
 constexpr int kTcStages = 2;
 constexpr int kTcMaxSlice = 1024;       // reduction indices per CTA (table entries held in shared memory)
 
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    // start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version = 1 [46,48) | layout_type = 0 (no swizzle) [61,64)
+__device__ __forceinline__ uint64_t gmma_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+    // start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | layout_type = 0 (no swizzle) [62,64).  No swizzle: LBO is
+    // the step between core matrices along K, SBO along M / N, for K-major and MN-major operands alike.
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3fff);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
-__device__ __forceinline__ uint32_t umma_instr_desc_bf16(int n, int a_mn_major, int b_mn_major) {
-    // c_format F32 [4,6) | a_format BF16 [7,10) | b_format BF16 [10,13) | a_major [15] | b_major [16] | N>>3 [17,23) |
-    // M>>4 [24,29)
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= 1u << 7;
-    d |= 1u << 10;
-    d |= (uint32_t)a_mn_major << 15;
-    d |= (uint32_t)b_mn_major << 16;
-    d |= (uint32_t)(n >> 3) << 17;
-    d |= (uint32_t)(kTcBM >> 4) << 24;
-    return d;
-}
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accum) {
+// D[64 x N] += A[64 x 16] * B[16 x N], bf16 operands from shared memory, fp32 accumulators in registers (the
+// m64nNk16 fragment: thread (warp w, lane l) of the warpgroup holds rows 16 w + l / 4 and 16 w + l / 4 + 8, columns
+// 8 j + 2 (l % 4) + {0, 1} in d[4 j .. 4 j + 3]).  kTA / kTB: the operand is MN-major (transposed), not K-major.
+template <int kTA, int kTB>
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t da, uint64_t db) {
     asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(d_tmem),
-        "l"(da), "l"(db), "r"(idesc), "r"(accum)
-        : "memory");
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %20, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, %18, %19;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "n"(kTA), "n"(kTB), "r"(1));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+template <int kTA, int kTB>
+__device__ __forceinline__ void wgmma_n64(float* d, uint64_t da, uint64_t db) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %36, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %34, %35;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "n"(kTA), "n"(kTB), "r"(1));
+}
+// one 64 x BN product: BN = 32 -> one n32 MMA, otherwise BN / 64 n64 MMAs on consecutive runs of eight column cores
+// of B (SBO = 128 bytes between column cores: the next 64 columns start 1024 bytes further)
+template <int BN, int kTA, int kTB>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db) {
+    static_assert(BN == 32 || BN % 64 == 0, "BN");
+    if constexpr (BN == 32) {
+        wgmma_n32<kTA, kTB>(d, da, db);
+    } else {
+#pragma unroll
+        for (int b = 0; b < BN / 64; ++b) wgmma_n64<kTA, kTB>(d + 32 * b, da, db + (uint64_t)(b * (1024 >> 4)));
+    }
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int N>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// accumulator fragments (MAIN + CORR) of a 64-row slab -> fp32 tile in shared memory, row stride ld floats
+template <int BN>
+__device__ __forceinline__ void store_fragment(float* tile, int ld, int r0, const float* main, const float* corr) {
+    const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+    const int row = r0 + 16 * w + (l >> 2);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = 8 * j + 2 * (l & 3);
+        *reinterpret_cast<float2*>(tile + (size_t)row * ld + col) =
+            make_float2(main[4 * j] + corr[4 * j], main[4 * j + 1] + corr[4 * j + 1]);
+        *reinterpret_cast<float2*>(tile + (size_t)(row + 8) * ld + col) =
+            make_float2(main[4 * j + 2] + corr[4 * j + 2], main[4 * j + 3] + corr[4 * j + 3]);
+    }
 }
 
 // 8 fp32 -> three 16-byte groups of bf16 (hi / mid / lo)
@@ -133,29 +162,18 @@ __device__ __forceinline__ bool tap_ok(int ri, int ci, int oh, int ow) {
     return y >= 0 && y < oh && x >= 0 && x < ow;
 }
 
-// thread = output row (TMEM lane): tcgen05.ld -> (1 / a_u8_div) -> bias / activation / activation-derivative mask ->
-// fp32 result (+ bf16 planes) or split-R partial
-#define CB200_TMEM_LD16(arr, addr)                                                                                   \
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];" \
-                 : "=r"(arr[0]), "=r"(arr[1]), "=r"(arr[2]), "=r"(arr[3]), "=r"(arr[4]), "=r"(arr[5]), "=r"(arr[6]),    \
-                   "=r"(arr[7]), "=r"(arr[8]), "=r"(arr[9]), "=r"(arr[10]), "=r"(arr[11]), "=r"(arr[12]),               \
-                   "=r"(arr[13]), "=r"(arr[14]), "=r"(arr[15])                                                          \
-                 : "r"(addr))
-
+// thread = output row of the accumulated tile (fp32 in shared memory, row stride ld) -> (1 / a_u8_div) -> bias /
+// activation / activation-derivative mask -> fp32 result (+ bf16 planes) or split-R partial
 template <int BN>
-__device__ __forceinline__ void tc_epilogue(const EpiParams& ep, uint32_t tmem_main, uint32_t tmem_corr, bool have_acc,
+__device__ __forceinline__ void tc_epilogue(const EpiParams& ep, const float* tile, int ld, bool have_acc,
                                             int m0, int n0, int M, int m_end, int N, int split, bool u8,
-                                            float a_u8_div, int unscaled_row, int col_lo = 0, int col_hi = BN,
-                                            uint32_t tmem_corr2 = 0xffffffffu) {
-    // tmem_corr2: a second accumulator of correction products (kCat scheme of nn_gemm_tiled.cuh): value = main +
-    // (corr + corr2)
-    // row = TMEM lane = thread index modulo 128 (a warp reaches the lane quadrant 32 * (warp % 4)); a second group
-    // of four warps may take the other half of the columns [col_lo, col_hi)
-    const int tid = threadIdx.x & 127, warp = tid >> 5;
+                                            float a_u8_div, int unscaled_row, int col_lo = 0, int col_hi = BN) {
+    // row = thread index modulo 128; a second group of four warps may take the other half of the columns
+    // [col_lo, col_hi)
+    const int tid = threadIdx.x & 127;
     const int m = m0 + tid;
     const bool scale_row = u8 && m != unscaled_row;
     const bool live = m < m_end;
-    const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
     // everything that depends only on the row (the asm memory clobbers below would otherwise force re-evaluation)
     const bool vec = !ep.accumulate && (N % 8 == 0);
     const size_t part_row = ((size_t)split * M + (live ? m : 0)) * N;
@@ -168,28 +186,21 @@ __device__ __forceinline__ void tc_epilogue(const EpiParams& ep, uint32_t tmem_m
         (ep.c_planes || ep.mask_planes) ? (p_row >> 3) * (size_t)(ep.c_plane_cols >> 3) * 64 + (p_row & 7) * 8 : 0;
 #pragma unroll 1
     for (int col = col_lo; col < col_hi; col += 16) {
-        uint32_t vm[16], vc[16];
+        if (!live) continue;
+        float v[16];
         if (have_acc) {
-            CB200_TMEM_LD16(vm, tmem_main + lane_base + (uint32_t)col);
-            CB200_TMEM_LD16(vc, tmem_corr + lane_base + (uint32_t)col);
-            if (tmem_corr2 != 0xffffffffu) {
-                uint32_t vd[16];
-                CB200_TMEM_LD16(vd, tmem_corr2 + lane_base + (uint32_t)col);
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            const float4* r = reinterpret_cast<const float4*>(tile + (size_t)tid * ld + col);
 #pragma unroll
-                for (int j = 0; j < 16; ++j) vc[j] = __float_as_uint(__uint_as_float(vc[j]) + __uint_as_float(vd[j]));
-            } else {
-                asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+            for (int j = 0; j < 4; ++j) {
+                const float4 q = r[j];
+                v[4 * j] = q.x; v[4 * j + 1] = q.y; v[4 * j + 2] = q.z; v[4 * j + 3] = q.w;
             }
         } else {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) vm[j] = vc[j] = 0u;
+            for (int j = 0; j < 16; ++j) v[j] = 0.f;
         }
-        if (!live) continue;
-        float v[16];
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-            v[j] = __uint_as_float(vm[j]) + __uint_as_float(vc[j]);
             if (scale_row) v[j] = __fdiv_rn(v[j], a_u8_div);
         }
 #pragma unroll
@@ -268,10 +279,16 @@ __device__ __forceinline__ void tc_epilogue(const EpiParams& ep, uint32_t tmem_m
     }
 }
 
+// the operand stages, reused for the fp32 accumulator tile [128][BN + 4] once the main loop is done
+template <int BN, bool kU8>
+__host__ __device__ constexpr size_t tc_region_bytes() {
+    constexpr size_t st = (size_t)kTcStages * ((kU8 ? 1 : 3) * kTcBM * kTcBK * 2 + 3 * BN * kTcBK * 2);
+    constexpr size_t tile = (size_t)kTcBM * (BN + 4) * sizeof(float);
+    return st > tile ? st : tile;
+}
 template <int BN, bool kU8>
 constexpr size_t tc_smem_bytes() {
-    return (size_t)kTcStages * ((kU8 ? 1 : 3) * kTcBM * kTcBK * 2 + 3 * BN * kTcBK * 2) + 64 + 1024 +
-           2 * kTcMaxSlice * sizeof(int32_t);
+    return tc_region_bytes<BN, kU8>() + 1024 + 2 * kTcMaxSlice * sizeof(int32_t);
 }
 
 // kU8: A is uint8 and contracted exactly (see the header); otherwise A is fp32, or uint8 through the LUT (general).
@@ -284,13 +301,11 @@ __global__ void __launch_bounds__(128) gemm_tc_kernel(FastA a, const float* __re
     constexpr int A_SPLIT = kTcBM * kTcBK * 2;            // bytes of one bf16 plane of the A chunk (8 KB)
     constexpr int B_SPLIT = BN * kTcBK * 2;
     constexpr int STAGE = NA * A_SPLIT + 3 * B_SPLIT;
-    constexpr int TMEM_COLS = (2 * BN <= 32) ? 32 : (2 * BN <= 64 ? 64 : (2 * BN <= 128 ? 128 : (2 * BN <= 256 ? 256 : 512)));
+    static_assert(BN <= 64, "one warpgroup holds the accumulators of both 64-row halves");
+    constexpr size_t REGION = tc_region_bytes<BN, kU8>();
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t* empty_bar = reinterpret_cast<uint64_t*>(smem + kTcStages * STAGE);      // [kTcStages]
-    uint64_t* done_bar = empty_bar + kTcStages;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
-    float* lut_s = reinterpret_cast<float*>(smem + kTcStages * STAGE + 64);          // 256 floats (uint8 via LUT)
-    int32_t* tab_off = reinterpret_cast<int32_t*>(smem + kTcStages * STAGE + 64 + 1024);
+    float* lut_s = reinterpret_cast<float*>(smem + REGION);                          // 256 floats (uint8 via LUT)
+    int32_t* tab_off = reinterpret_cast<int32_t*>(smem + REGION + 1024);
     int32_t* tab_info = tab_off + kTcMaxSlice;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -300,16 +315,6 @@ __global__ void __launch_bounds__(128) gemm_tc_kernel(FastA a, const float* __re
     const int r_hi = min(R, r_lo + r_per_split);
     const bool has_info = a.rowinfo != nullptr;
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-    if (tid == 0) {
-        for (int s = 0; s < kTcStages; ++s) mbar_init(empty_bar + s, 1);
-        mbar_init(done_bar, 1);
-        fence_mbar_init();
-    }
     if (!kU8 && a.lut) {
         for (int i = tid; i < 256; i += 128) lut_s[i] = a.lut[i];
     }
@@ -326,13 +331,8 @@ __global__ void __launch_bounds__(128) gemm_tc_kernel(FastA a, const float* __re
             if (has_info) tab_info[j] = __ldg(a.rowinfo + r_lo + j);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
     if (!kU8 && a.lut) a.lut = lut_s;
-    const uint32_t tmem_main = *tmem_slot;
-    const uint32_t tmem_corr = tmem_main + BN;            // column offset
-    const uint32_t idesc = umma_instr_desc_bf16(BN, kTransA ? 1 : 0, 1);
 
     // ---- per-thread constants of the A loader ---------------------------------------------------------------------
     // K-major item (row, k-group of 8 = two gather groups of 4): lane l of warp w handles k-group l >> 3 of rows
@@ -506,50 +506,63 @@ __global__ void __launch_bounds__(128) gemm_tc_kernel(FastA a, const float* __re
         }
     };
 
+    // accumulators of the two 64-row halves of the tile: MAIN collects a1*b1, CORR the correction products
+    float acc[2][2][BN / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) acc[h][0][j] = acc[h][1][j] = 0.f;
+    constexpr int kTA = kTransA ? 1 : 0;
     if (nchunks > 0) fetch(0);
     for (int c = 0; c < nchunks; ++c) {
-        const int s = c % kTcStages, use = c / kTcStages;
+        const int s = c % kTcStages;
         uint8_t* sA = smem + s * STAGE;
         uint8_t* sB = sA + NA * A_SPLIT;
-        if (use > 0) mbar_wait(empty_bar + s, (uint32_t)((use - 1) & 1));     // MMAs that read this stage are done
+        // the MMAs of chunk c - 2 read this stage: at most the group of chunk c - 1 may still be in flight
+        wgmma_wait<kTcStages - 1>();
         convert_store(sA, sB);
         if (c + 1 < nchunks) fetch(c + 1);
         fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core (async proxy)
         __syncthreads();
-        if (tid == 0) {
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            constexpr uint32_t A_LBO = (kTcBM / 8) * 128, B_LBO = (BN / 8) * 128, SBO = 128;
-            const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
+        wgmma_fence();
+        constexpr uint32_t A_LBO = (kTcBM / 8) * 128, B_LBO = (BN / 8) * 128, SBO = 128;
+        const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
 #pragma unroll
-            for (int ks = 0; ks < kTcBK / 16; ++ks) {
-                const uint32_t ao = ks * 2 * A_LBO, bo = ks * 2 * B_LBO;
-                auto desc_a = [&](int sp) { return umma_smem_desc(a_base + sp * A_SPLIT + ao, A_LBO, SBO); };
-                auto desc_b = [&](int sp) { return umma_smem_desc(b_base + sp * B_SPLIT + bo, B_LBO, SBO); };
-                const uint32_t first = (c == 0 && ks == 0) ? 0u : 1u;
-                umma_bf16(tmem_main, desc_a(0), desc_b(0), idesc, first);          // a1 b1
-                umma_bf16(tmem_corr, desc_a(0), desc_b(2), idesc, first);          // a1 b3
+        for (int ks = 0; ks < kTcBK / 16; ++ks) {
+            const uint32_t ao = ks * 2 * A_LBO, bo = ks * 2 * B_LBO;
+            auto desc_b = [&](int sp) { return gmma_smem_desc(b_base + sp * B_SPLIT + bo, B_LBO, SBO); };
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                // rows 64 h .. 64 h + 63: eight 8-row core groups further (SBO = 128 bytes apart)
+                auto desc_a = [&](int sp) { return gmma_smem_desc(a_base + sp * A_SPLIT + ao + h * 1024, A_LBO, SBO); };
+                float* mn = acc[h][0];
+                float* cr = acc[h][1];
+                wgmma_tile<BN, kTA, 1>(mn, desc_a(0), desc_b(0));             // a1 b1
+                wgmma_tile<BN, kTA, 1>(cr, desc_a(0), desc_b(2));             // a1 b3
                 if (!kU8) {
-                    umma_bf16(tmem_corr, desc_a(2), desc_b(0), idesc, 1u);         // a3 b1
-                    umma_bf16(tmem_corr, desc_a(1), desc_b(1), idesc, 1u);         // a2 b2
+                    wgmma_tile<BN, kTA, 1>(cr, desc_a(2), desc_b(0));         // a3 b1
+                    wgmma_tile<BN, kTA, 1>(cr, desc_a(1), desc_b(1));         // a2 b2
                 }
-                umma_bf16(tmem_corr, desc_a(0), desc_b(1), idesc, 1u);             // a1 b2
-                if (!kU8) umma_bf16(tmem_corr, desc_a(1), desc_b(0), idesc, 1u);   // a2 b1
+                wgmma_tile<BN, kTA, 1>(cr, desc_a(0), desc_b(1));             // a1 b2
+                if (!kU8) wgmma_tile<BN, kTA, 1>(cr, desc_a(1), desc_b(0));   // a2 b1
             }
-            umma_commit(empty_bar + s);
-            if (c == nchunks - 1) umma_commit(done_bar);
         }
+        wgmma_commit();
     }
-    if (nchunks > 0) {
-        mbar_wait(done_bar, 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        acc_fence<BN / 2>(acc[h][0]);
+        acc_fence<BN / 2>(acc[h][1]);
     }
-    tc_epilogue<BN>(ep, tmem_main, tmem_corr, nchunks > 0, m0, n0, M, M, N, split, kU8, a_u8_div,
-                    (kU8 && kTransA) ? a.ones_col : -1);
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    __syncthreads();                       // every MMA of the CTA is complete: the stages become the result tile
+    float* tile = reinterpret_cast<float*>(smem);
+    constexpr int LD = BN + 4;
+    store_fragment<BN>(tile, LD, 0, acc[0][0], acc[0][1]);
+    store_fragment<BN>(tile, LD, 64, acc[1][0], acc[1][1]);
     __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_main), "r"(TMEM_COLS));
-    }
+    tc_epilogue<BN>(ep, tile, LD, nchunks > 0, m0, n0, M, M, N, split, kU8, a_u8_div,
+                    (kU8 && kTransA) ? a.ones_col : -1);
 }
 
 }  // namespace gemm

@@ -16,18 +16,19 @@
 //
 // A CTA owns one 128 x BN output tile: 128 consecutive batch rows of one pixel (mode 0) or 128 rows of the stacked
 // per-tap weight matrix (mode 1).  Because of the plane format every operand chunk (32 reduction indices) is a few
-// contiguous runs of 128-byte core matrices, so the PRODUCER warp moves it with 1-D bulk copies (cp.async.bulk,
-// completion counted in bytes on an mbarrier -- the TMA engine, no registers, no shared-memory stores by threads), the
-// MMA warp (one elected thread) issues the 3xBF16 product set of nn_gemm_tc.cuh as soon as the "full" barrier of a
-// stage flips and releases the stage through tcgen05.commit -> "empty" barrier, and the four EPILOGUE warps drain
-// the TMEM accumulators at the end (tc_epilogue: bias / activation / derivative mask, fp32 result + planes).
+// contiguous runs of 128-byte core matrices, so the PRODUCER warp moves it with TMA (tensor-map boxes or 1-D bulk
+// copies, completion counted in bytes on an mbarrier -- no registers, no shared-memory stores by threads).  Two
+// CONSUMER warpgroups (rows 0-63 and 64-127 of the tile) issue the 3xBF16 product set of nn_gemm_tc.cuh with wgmma as
+// soon as the "full" barrier of a stage flips, keep the fp32 accumulators in registers and release a stage on its
+// "empty" barrier once wgmma.wait_group reports its MMAs complete.  At the end they stage the accumulators through
+// shared memory and run tc_epilogue (bias / activation / derivative mask, fp32 result + planes).
 //
 // Tensor maps.  A plane set is a 4-D bf16 tensor (64 elements of a core | cores per 8-row group | row groups | 3
 // planes); one TMA tile operation with box (64, cores, row groups, 3) fetches the hi / mid / lo planes of a whole
 // operand chunk and lands them densely -- exactly the layouts below.  Mode 0 needs TWO operations per chunk (A, B),
 // mode 1 one for G plus 1-D bulk copies for the A^T runs (one per tap and 8-row group: taps sit at unrelated pixels
-// and the M direction must stay uniformly strided in shared memory).  A TMA operation costs ~60 cycles of issue on
-// an SM whatever its size (measured, profiles/), which is what makes few large operations matter.
+// and the M direction must stay uniformly strided in shared memory).  Few large TMA operations keep the single
+// producer warp's issue cost low.
 //
 // Shared-memory operand layouts (no swizzle; LBO = step between core matrices along K, SBO = along M / N):
 //   A  K-major  [128 rows, 32 k] : core (rg, kg) at rg * 512 + kg * 128          LBO = 128,  SBO = 512
@@ -40,19 +41,6 @@
 
 namespace cb200 {
 namespace gemm {
-
-#ifdef CB200_TC_PROF
-// build-time instrumentation (CB200_EXTRA_NVCC_FLAGS=-DCB200_TC_PROF python -m coach_b200.build --force): cycles the
-// producer lane 0 / the MMA thread / epilogue thread 0 of CTA (0,0,0) spend per phase; read with cb200_tc_prof_read
-// (tools/tc_phase_probe.py)
-__device__ unsigned long long g_tc_prof[16];
-#define TC_PROF_T(var) const long long var = clock64()
-#define TC_PROF_ADD(i, a, b) \
-    if (prof_on) g_tc_prof[i] += (unsigned long long)((b) - (a))
-#else
-#define TC_PROF_T(var)
-#define TC_PROF_ADD(i, a, b)
-#endif
 
 struct TiledParams {
     int mode;
@@ -75,15 +63,18 @@ struct TiledParams {
 };
 
 // NA = planes of the A operand: 3 (fp32 split) or 1 (uint8 values, exact: 3 products instead of 6)
-// warps 0-7: epilogue (two per TMEM lane quadrant, half of the tile's columns each; in mode 1 they also help issuing
-// bulk copies during the main loop), warp 8: producer, warp 9: MMA issuer
-constexpr int kTlThreads = 320;
-constexpr int kTlProducerWarp = 8, kTlMmaWarp = 9;
+// warps 0-7: two consumer warpgroups (rows 0-63 and 64-127 of the tile: wgmma, then the epilogue with half of the
+// tile's columns per group of four warps), warp 8: producer
+constexpr int kTlThreads = 288;
+constexpr int kTlProducerWarp = 8;
+constexpr int kTlConsumers = 256;
 
 template <int BN, int NA>
 struct TiledCfg {
     static constexpr int kStages = BN == 128 ? 4 : 3;
-    static constexpr size_t kSmemBytes = (size_t)kStages * (NA * kTcBM * kTcBK * 2 + 3 * BN * kTcBK * 2) + 128 + 4096;
+    static constexpr size_t kStageRegion = (size_t)kStages * (NA * kTcBM * kTcBK * 2 + 3 * BN * kTcBK * 2);
+    static_assert(kStageRegion >= (size_t)kTcBM * (BN + 4) * sizeof(float), "result tile overlays the stages");
+    static constexpr size_t kSmemBytes = kStageRegion + 128 + 1024;
 };
 
 __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, int c4,
@@ -104,14 +95,15 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         : "memory");
 }
 
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kTlConsumers) : "memory"); }
+
 // tmA: planes of A with box (64, 4, 16, NA) (mode 0 only); tmB: planes of the B operand with box (64, BN / 8, 4, 3)
-// kCat (mode 0, BN <= 64, row-group interleaved B planes): the B box lands as [k-group][plane][column core], one
-// MN-major operand [32 k, 3 BN] = [b1 | b2 | b3].  The product set becomes THREE tcgen05.mma per k16 step,
-//     a1 x [b1|b2|b3] (N = 3 BN) -> columns MAIN | CA | CB       a2 x [b1|b2] (N = 2 BN) -> CA | CB
-//     a3 x [b1]       (N = BN)   -> CA                            value = MAIN + (CA + CB)
-// i.e. the same six products with each A plane read from shared memory once per k-step instead of 3 / 2 / 1 times: an
-// SS-mode MMA of width 64 reads (128 + 64) x 16 x 2 B = 6 KB per 32 tensor cycles, 192 B/cycle against the 128 B/cycle
-// shared memory delivers -- the six narrow MMAs were bound by shared-memory reads, not by the tensor pipe.
+// kCat (mode 0, BN <= 64, row-group interleaved B planes): the B box lands as [k-group][plane][column core]; each
+// plane is then an MN-major operand with k-group stride 3 * (BN / 8) * 128 bytes, and the six narrow products are
+// issued on it as on separate planes.  The interleaved operand would also allow three wide MMAs on one MAIN | CA | CB
+// fragment (a1 x [b1|b2|b3] at N = 3 BN, a2 x [b1|b2], a3 x b1), reading each A plane once per k-step; measured on an
+// H100 SXM (700 W) in the DQN step that form took 760 us of tiled-GEMM time per step against 724-727 us for the six
+// narrow wgmma, so it is not used.
 template <int BN, bool kTransA, int NA, bool kCat = false>
 __global__ void __launch_bounds__(kTlThreads) gemm_tc_tiled_kernel(const __grid_constant__ CUtensorMap tmA,
                                                             const __grid_constant__ CUtensorMap tmB,
@@ -123,21 +115,18 @@ __global__ void __launch_bounds__(kTlThreads) gemm_tc_tiled_kernel(const __grid_
     constexpr int B_SPLIT = BN * kTcBK * 2;
     constexpr int STAGE = NA * A_SPLIT + 3 * B_SPLIT;
     constexpr int B_KG = (BN / 8) * 128;                  // bytes of one k-group (8 reduction rows) of the B tile
+    constexpr size_t REGION = TiledCfg<BN, NA>::kStageRegion;
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S * STAGE);     // [S]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + REGION);       // [S]
     uint64_t* empty_bar = full_bar + S;                                    // [S]
-    uint64_t* done_bar = empty_bar + S;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
-    uint8_t* ones_tile = smem + S * STAGE + 128;          // 4 KB: a [128 x 16] A^T operand of bf16 1.0 (bias row)
+    float* bias_part = reinterpret_cast<float*>(smem + REGION + 128);      // [256] partial column sums (bias row)
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    // Bias gradient (mode 1): the CTAs of the first M tile also accumulate ones^T * G in two more TMEM accumulators --
-    // every row of that product is sum_rows G[row, :], the epilogue keeps row 0.  Three extra MMAs per k16 step in
-    // 1 / gridDim.x of the CTAs replace a separate column-sum pass over dY.
+    // Bias gradient (mode 1): the CTAs of the first M tile also form sum_rows G[row, :] -- the consumer threads add
+    // the three exact bf16 planes of every G chunk in fp32 while the tensor core works on it.  This replaces a
+    // separate column-sum pass over dY.
     const bool bias_cta = kTransA && tp.bias_row != 0 && blockIdx.x == 0;
     static_assert(!kCat || (!kTransA && BN <= 64), "kCat: mode 0, BN <= 64");
-    const uint32_t tmem_cols_needed = kCat ? 3u * BN : (bias_cta ? 4u : 2u) * BN;
-    const uint32_t TMEM_COLS = tmem_cols_needed <= 32 ? 32u : (tmem_cols_needed <= 64 ? 64u : (tmem_cols_needed <= 128 ? 128u : (tmem_cols_needed <= 256 ? 256u : 512u)));
     const int B = tp.batch, Ca = tp.a_cols, N = tp.n;
     const int n0 = blockIdx.y * BN;
     const int split = blockIdx.z;
@@ -163,40 +152,17 @@ __global__ void __launch_bounds__(kTlThreads) gemm_tc_tiled_kernel(const __grid_
     const int c_hi = min(total, c_lo + tp.chunks_per_split);
     const int nchunks = max(0, c_hi - c_lo);
 
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                     "r"(TMEM_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
     if (tid == 0) {
         for (int s = 0; s < S; ++s) {
             mbar_init(full_bar + s, 1);
-            mbar_init(empty_bar + s, 1);
+            mbar_init(empty_bar + s, kTlConsumers / 32);   // one elected lane of each consumer warp
         }
-        mbar_init(done_bar, 1);
         fence_mbar_init();
     }
-    if (bias_cta && tid < 128) {     // (any 128 threads)
-        // 2048 bf16 ones, 16 per thread; generic-proxy stores made visible to the tensor core (async proxy)
-        uint4* o = reinterpret_cast<uint4*>(ones_tile) + 2 * tid;
-        o[0] = o[1] = make_uint4(0x3F803F80u, 0x3F803F80u, 0x3F803F80u, 0x3F803F80u);
-        fence_proxy_async_smem();
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_main = *tmem_slot;
-    const uint32_t tmem_corr = tmem_main + BN;
-    const uint32_t tmem_bias_main = tmem_main + 2 * BN, tmem_bias_corr = tmem_main + 3 * BN;
-#ifdef CB200_TC_PROF
-    const bool cta0 = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
-#endif
 
     if (warp == kTlProducerWarp) {
         // ================= producer: bulk copies of the operand cores into the stage ring =========================
-#ifdef CB200_TC_PROF
-        const bool prof_on = cta0 && lane == 0;
-#endif
         // mode 1: taps covered by this M tile, and the channel range inside a tap
         const int taps_in_tile = kTransA ? (Ca >= kTcBM ? 1 : min(kTcBM / Ca, tp.taps - m0 / Ca)) : 0;
         const int t0 = kTransA ? m0 / Ca : 0;
@@ -214,9 +180,7 @@ __global__ void __launch_bounds__(kTlThreads) gemm_tc_tiled_kernel(const __grid_
         }
         for (int j = 0; j < nchunks; ++j) {
             const int s = j % S, u = j / S;
-            TC_PROF_T(t0c);
             if (u > 0) mbar_wait(empty_bar + s, (uint32_t)((u - 1) & 1));      // MMAs that read this stage are done
-            TC_PROF_T(t1c);
             uint8_t* sA = smem + s * STAGE;
             uint8_t* sB = sA + NA * A_SPLIT;
             uint64_t* bar = full_bar + s;
@@ -243,10 +207,8 @@ __global__ void __launch_bounds__(kTlThreads) gemm_tc_tiled_kernel(const __grid_
                     }
                     continue;
                 }
-                // A^T: per tap of the tile, 4 k-groups (8 batch rows each) x a run of cw / 8 cores.  A bulk copy costs
-                // ~60 cycles of issue in the issuing warp whatever its size, so the runs are dealt out over nine
-                // warps: this one and the eight epilogue warps, which are idle until the accumulators are complete.
-                for (int idx = lane; idx < NA * 4 * taps_in_tile; idx += 9 * 32) {
+                // A^T: per tap of the tile, 4 k-groups (8 batch rows each) x a run of cw / 8 cores
+                for (int idx = lane; idx < NA * 4 * taps_in_tile; idx += 32) {
                     const int p = idx / (4 * taps_in_tile), r = idx % (4 * taps_in_tile);
                     const int tt = r >> 2, kg = r & 3;
                     const int apix = __ldg(tp.a_pix + (size_t)(t0 + tt) * tp.num_q + qq);
@@ -256,145 +218,90 @@ __global__ void __launch_bounds__(kTlThreads) gemm_tc_tiled_kernel(const __grid_
                              (uint32_t)((cw >> 3) * 128), bar);
                 }
             }
-            TC_PROF_T(t2c);
-            TC_PROF_ADD(0, t0c, t1c);      // producer: wait for a free stage
-            TC_PROF_ADD(1, t1c, t2c);      // producer: issue the copies
-            TC_PROF_ADD(2, t0c - 1, t0c);  // chunk count
-        }
-    } else if (warp == kTlMmaWarp) {
-        // ================= MMA issuer ===============================================================================
-#ifdef CB200_TC_PROF
-        const bool prof_on = cta0 && lane == 0;
-#endif
-        const uint32_t idesc = umma_instr_desc_bf16(BN, kTransA ? 1 : 0, 1);
-        constexpr uint32_t A_LBO = kTransA ? 2048u : 128u, A_SBO = kTransA ? 128u : 512u;
-        constexpr uint32_t A_KS = kTransA ? 2u * 2048u : 256u;                 // bytes per k16 step
-        constexpr uint32_t B_LBO = (uint32_t)B_KG, B_SBO = 128u, B_KS = 2u * (uint32_t)B_KG;
-        const uint64_t a_hi = umma_smem_desc(0u, A_LBO, A_SBO), b_hi = umma_smem_desc(0u, B_LBO, B_SBO);
-        const uint32_t smem_base = smem_u32(smem);
-        for (int j = 0; j < nchunks; ++j) {
-            const int s = j % S, u = j / S;
-            TC_PROF_T(t0m);
-            mbar_wait(full_bar + s, (uint32_t)(u & 1));                        // the bulk copies of this stage landed
-            TC_PROF_T(t1m);
-            if (lane == 0) {
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t a_base = smem_base + s * STAGE, b_base = a_base + NA * A_SPLIT;
-#pragma unroll
-                for (int ks = 0; ks < kTcBK / 16; ++ks) {
-                    const uint64_t a0 = a_hi | (uint64_t)((a_base + ks * A_KS) >> 4);
-                    const uint64_t a1 = a0 + (A_SPLIT >> 4), a2 = a0 + 2 * (A_SPLIT >> 4);
-                    const uint32_t first = (j == 0 && ks == 0) ? 0u : 1u;
-                    if (kCat) {
-                        // B stage = [k-group][plane][column core]: k-group stride 3 * B_KG, column-core stride 128
-                        const uint64_t bd = umma_smem_desc(b_base + ks * 2u * 3u * (uint32_t)B_KG, 3u * (uint32_t)B_KG, 128u);
-                        umma_bf16(tmem_main, a0, bd, umma_instr_desc_bf16(3 * BN, 0, 1), first);   // a1 [b1|b2|b3]
-                        if (NA == 3) {
-                            umma_bf16(tmem_main + BN, a1, bd, umma_instr_desc_bf16(2 * BN, 0, 1), 1u);   // a2 [b1|b2]
-                            umma_bf16(tmem_main + BN, a2, bd, umma_instr_desc_bf16(BN, 0, 1), 1u);       // a3 [b1]
-                        }
-                        continue;
-                    }
-                    const uint64_t b0d = b_hi | (uint64_t)((b_base + ks * B_KS) >> 4);
-                    const uint64_t b1 = b0d + (B_SPLIT >> 4), b2 = b0d + 2 * (B_SPLIT >> 4);
-                    umma_bf16(tmem_main, a0, b0d, idesc, first);       // a1 b1
-                    umma_bf16(tmem_corr, a0, b2, idesc, first);        // a1 b3
-                    if (NA == 3) {
-                        umma_bf16(tmem_corr, a2, b0d, idesc, 1u);      // a3 b1
-                        umma_bf16(tmem_corr, a1, b1, idesc, 1u);       // a2 b2
-                    }
-                    umma_bf16(tmem_corr, a0, b1, idesc, 1u);           // a1 b2
-                    if (NA == 3) umma_bf16(tmem_corr, a1, b0d, idesc, 1u);   // a2 b1
-                    if (bias_cta) {
-                        const uint64_t od = umma_smem_desc(smem_u32(ones_tile), 2048u, 128u);
-                        umma_bf16(tmem_bias_main, od, b0d, idesc, first);      // 1 g1
-                        umma_bf16(tmem_bias_corr, od, b2, idesc, first);       // 1 g3
-                        umma_bf16(tmem_bias_corr, od, b1, idesc, 1u);          // 1 g2
-                    }
-                }
-                umma_commit(empty_bar + s);
-                if (j == nchunks - 1) umma_commit(done_bar);
-            }
-            __syncwarp();
-            TC_PROF_T(t2m);
-            TC_PROF_ADD(3, t0m, t1m);      // MMA thread: wait for data
-            TC_PROF_ADD(4, t1m, t2m);      // MMA thread: issue
         }
     } else {
-        // ================= epilogue warps (TMEM lanes 0..127) =====================================================
-#ifdef CB200_TC_PROF
-        const bool prof_on = cta0 && tid == 0;
-#endif
-        if (kTransA) {
-            // main loop: help the producer with the A^T bulk copies (slots 1..8 of the nine-way deal)
-            const int taps_in_tile = Ca >= kTcBM ? 1 : min(kTcBM / Ca, tp.taps - m0 / Ca);
-            const int t0 = m0 / Ca, cw = min(Ca, kTcBM), c0 = m0 % Ca;
-            for (int j = 0; j < nchunks; ++j) {
-                const int s = j % S, u = j / S;
-                if (tp.a_tma != 0 || (warp + 1) * 32 >= NA * 4 * taps_in_tile) break;   // nothing dealt to this warp
-                if (u > 0) mbar_wait(empty_bar + s, (uint32_t)((u - 1) & 1));
-                uint8_t* sA = smem + s * STAGE;
-                uint64_t* bar = full_bar + s;
-                const int cj = c_lo + j;
-                const int qq = cj / bc_per, bc = cj % bc_per;
-                for (int idx = (warp + 1) * 32 + lane; idx < NA * 4 * taps_in_tile; idx += 9 * 32) {
-                    const int p = idx / (4 * taps_in_tile), r = idx % (4 * taps_in_tile);
-                    const int tt = r >> 2, kg = r & 3;
-                    const int apix = __ldg(tp.a_pix + (size_t)(t0 + tt) * tp.num_q + qq);
-                    const size_t rg = (((size_t)apix * B + (size_t)bc * kTcBK) >> 3) + kg;
-                    bulk_g2s(sA + p * A_SPLIT + kg * 2048 + tt * (Ca >> 3) * 128,
-                             tp.a + p * tp.a_stride + (rg * (size_t)(Ca >> 3) + (size_t)(c0 >> 3)) * 64,
-                             (uint32_t)((cw >> 3) * 128), bar);
+        // ================= consumers: warpgroup g computes rows 64 g .. 64 g + 63 of the tile =====================
+        const int g = warp >> 2;
+        constexpr int kTA = kTransA ? 1 : 0;
+        // A K-major  [128 rows, 32 k]: core (rg, kg) at rg * 512 + kg * 128   -> rows 64 g start 8 * 512 g further
+        // A^T MN-major [128 m, 32 k]: core (kg, mg) at kg * 2048 + mg * 128   -> rows 64 g start 8 * 128 g further
+        constexpr uint32_t A_LBO = kTransA ? 2048u : 128u, A_SBO = kTransA ? 128u : 512u;
+        constexpr uint32_t A_KS = kTransA ? 2u * 2048u : 256u;                 // bytes per k16 step
+        const uint32_t a_half = (uint32_t)g * 8u * A_SBO;
+        // B MN-major: k-group stride B_KG (plane stride B_SPLIT), or 3 * B_KG (plane stride B_KG) when interleaved
+        constexpr uint32_t B_LBO = kCat ? 3u * (uint32_t)B_KG : (uint32_t)B_KG;
+        constexpr uint32_t B_PLANE = kCat ? (uint32_t)B_KG : (uint32_t)B_SPLIT;
+        const uint32_t smem_base = smem_u32(smem);
+        float mn[BN / 2], cr[BN / 2];
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) mn[j] = cr[j] = 0.f;
+        // bias row: thread t sums column t % BN over the reduction rows kk = t / BN (mod 256 / BN)
+        float bsum = 0.f;
+        const int bcol = tid % BN, brow0 = tid / BN;
+        for (int j = 0; j < nchunks; ++j) {
+            const int s = j % S, u = j / S;
+            mbar_wait(full_bar + s, (uint32_t)(u & 1));                        // the bulk copies of this stage landed
+            const uint32_t a_base = smem_base + s * STAGE + a_half, b_base = smem_base + s * STAGE + NA * A_SPLIT;
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < kTcBK / 16; ++ks) {
+                const uint64_t a0 = gmma_smem_desc(a_base + ks * A_KS, A_LBO, A_SBO);
+                const uint64_t a1 = a0 + (A_SPLIT >> 4), a2 = a0 + 2 * (A_SPLIT >> 4);
+                const uint64_t b0d = gmma_smem_desc(b_base + ks * 2u * B_LBO, B_LBO, 128u);
+                const uint64_t b1 = b0d + (B_PLANE >> 4), b2 = b0d + 2 * (B_PLANE >> 4);
+                wgmma_tile<BN, kTA, 1>(mn, a0, b0d);           // a1 b1
+                wgmma_tile<BN, kTA, 1>(cr, a0, b2);            // a1 b3
+                if (NA == 3) {
+                    wgmma_tile<BN, kTA, 1>(cr, a2, b0d);       // a3 b1
+                    wgmma_tile<BN, kTA, 1>(cr, a1, b1);        // a2 b2
                 }
-                __syncwarp();
+                wgmma_tile<BN, kTA, 1>(cr, a0, b1);            // a1 b2
+                if (NA == 3) wgmma_tile<BN, kTA, 1>(cr, a1, b0d);   // a2 b1
             }
+            wgmma_commit();
+            if (bias_cta) {
+                const uint16_t* sb = reinterpret_cast<const uint16_t*>(smem + s * STAGE + NA * A_SPLIT);
+                for (int kk = brow0; kk < kTcBK; kk += kTlConsumers / BN) {
+                    const int e = ((kk >> 3) * B_KG + (bcol >> 3) * 128 + (kk & 7) * 16) / 2 + (bcol & 7);
+                    const float g1 = __uint_as_float((uint32_t)sb[e] << 16);
+                    const float g2 = __uint_as_float((uint32_t)sb[e + B_SPLIT / 2] << 16);
+                    const float g3 = __uint_as_float((uint32_t)sb[e + B_SPLIT] << 16);
+                    bsum += g1 + g2 + g3;
+                }
+            }
+            // the MMAs of chunk j - 1 are complete: release its stage
+            wgmma_wait<1>();
+            __syncwarp();
+            if (j > 0 && lane == 0)
+                asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(empty_bar + (j - 1) % S))
+                             : "memory");
         }
-        TC_PROF_T(t0e);
-        if (nchunks > 0) {
-            mbar_wait(done_bar, 0);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        TC_PROF_T(t1e);
+        wgmma_wait<0>();
+        acc_fence<BN / 2>(mn);
+        acc_fence<BN / 2>(cr);
+        consumer_sync();                   // every MMA of the tile is complete: the stages become the result tile
+        float* tile = reinterpret_cast<float*>(smem);
+        constexpr int LD = BN + 4;
+        store_fragment<BN>(tile, LD, 64 * g, mn, cr);
+        if (bias_cta) bias_part[tid] = bsum;
+        consumer_sync();
         {
             const int half = warp >> 2;                        // warps 0-3: low half of the columns, 4-7: high half
-            tc_epilogue<BN>(ep, tmem_main, tmem_corr, nchunks > 0, m0, n0, M, m_end, N, split, NA == 1, tp.a_u8_div, -1,
-                            half * (BN / 2), half * (BN / 2) + BN / 2, kCat ? tmem_main + 2 * BN : 0xffffffffu);
+            tc_epilogue<BN>(ep, tile, LD, nchunks > 0, m0, n0, M, m_end, N, split, NA == 1, tp.a_u8_div, -1,
+                            half * (BN / 2), half * (BN / 2) + BN / 2);
         }
-        if (bias_cta && warp == 0) {
-            // row `m_end` (= taps * Ca) of the result: lane 0 owns TMEM lane 0 of the bias accumulators
-#pragma unroll 1
-            for (int col = 0; col < BN; col += 16) {
-                uint32_t vm[16], vc[16];
-                if (nchunks > 0) {
-                    CB200_TMEM_LD16(vm, tmem_bias_main + (uint32_t)col);
-                    CB200_TMEM_LD16(vc, tmem_bias_corr + (uint32_t)col);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) vm[j] = vc[j] = 0u;
-                }
-                if (lane == 0) {
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int n = n0 + col + j;
-                        if (n >= N) continue;
-                        const float v = __uint_as_float(vm[j]) + __uint_as_float(vc[j]);
-                        if (ep.splits > 1)
-                            ep.partial[((size_t)split * M + m_end) * N + n] = v;
-                        else
-                            epilogue_store(ep, m_end, n, v);
-                    }
-                }
+        if (bias_cta && tid < BN) {
+            // row `m_end` (= taps * Ca) of the result
+            const int n = n0 + tid;
+            float v = 0.f;
+            for (int r = 0; r < kTlConsumers / BN; ++r) v += bias_part[r * BN + tid];
+            if (n < N) {
+                if (ep.splits > 1)
+                    ep.partial[((size_t)split * M + m_end) * N + n] = v;
+                else
+                    epilogue_store(ep, m_end, n, v);
             }
         }
-        TC_PROF_T(t2e);
-        TC_PROF_ADD(5, t0e, t1e);          // main loop as seen by the epilogue warps
-        TC_PROF_ADD(6, t1e, t2e);          // epilogue
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_main), "r"(TMEM_COLS));
     }
 }
 

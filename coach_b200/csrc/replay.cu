@@ -1295,8 +1295,8 @@ static int launch_gather_s2d(const SampleParams& sp, const int64_t* idx_in, int6
     memset(&tmF, 0, sizeof(tmF));
     // frame store, opt-in (cb200_tune("frame_tma", 1)): per-sample stage regions 128 bytes apart in alignment (TMA box
     // destination) when the tensor map can be built; otherwise (and for the verbatim ring) the padded odd-multiple-of-
-    // 16 stride of the bulk-copy path.  Measured (profiles/README.md r2i): 49.5 us with the boxes, 50.7 us with four
-    // bulk copies per stack -- the kernel is not bound by the number of copy requests -- so the simpler path is default.
+    // 16 stride of the bulk-copy path.  The kernel is not bound by the number of copy requests, so the simpler path is
+    // the default.
     gp.frame_tma = frames && frame_slots >= 4 && stride % 128 == 0 && tune_get("frame_tma", 0, 0, 1) != 0 &&
                    frame_store_map(&tmF, frames, (int64_t)h * w, frame_slots, rc * s * w);
     if (!gp.frame_tma && (stride / 16) % 2 == 0) stride += 16;

@@ -6,7 +6,7 @@ and converts AoS -> SoA on every sample (core_types.py:488-623).  Here every tra
 (``cb200_gather`` / ``cb200_per_sample_gather``), an append is a row scatter (``cb200_scatter_ring``).
 
 Layout for the Atari configuration (2^20 slots): state 28,224 B + next_state 28,224 B + action 8 B + reward 8 B +
-game_over 1 B per slot = 59.2 GB, sized for the 180 GB of a B200.
+game_over 1 B per slot = 59.2 GB, which fits the 80 GB of an H100.
 
 Frame-deduplicated mode (``declare_schema(..., frame_stack=[...])``, SURVEY.md 8(f1)): a stacked image observation
 [H, W, K] is K frames of which K-1 also belong to the neighbouring transitions -- the reference shares them by

@@ -1,5 +1,5 @@
 /*
- * include/coach_b200.h -- C ABI of libcoach_b200.so (hand-written sm_100a CUDA behind Coach's
+ * include/coach_b200.h -- C ABI of libcoach_b200.so (hand-written sm_90a CUDA behind Coach's
  * replay-sample -> learn_from_batch hot path).
  *
  * The reference (IntelLabs/coach, rl-coach 1.0.1) is pure Python and has no FFI of its own; its plugin boundary is
@@ -36,11 +36,11 @@ const char* cb200_last_error(void);
 int64_t cb200_launch_count(void);
 /* Multiprocessor count and compute capability of the current device (any pointer may be NULL). */
 int cb200_device_info(int* sm_count, int* cc_major, int* cc_minor);
-/* Runtime switches for benchmark A/B runs (unknown keys are stored and ignored):
+/* Runtime switches for benchmark A/B runs (unknown keys are stored and ignored; the removed key "gemm_persistent" --
+ * the persistent schedule of cb200_gemm_tiled -- is rejected with CB200_ERR_INVALID_ARGUMENT):
  *   "gather_ctas_per_sm" (persistent gather grid = SMs x this, default 4), "gather_stages" (0 = automatic)
- *   "gemm_tc" (1)          tcgen05 path of cb200_gemm; 0 = fp32 CUDA-core kernels only
- *   "gemm_skinny" (1)      dedicated kernels for products with n <= 8 or k <= 8
- *   "gemm_persistent" (0)  persistent schedule of cb200_gemm_tiled (two TMEM accumulator sets, 8 epilogue warps) */
+ *   "gemm_tc" (1)          tensor-core (wgmma) path of cb200_gemm; 0 = fp32 CUDA-core kernels only
+ *   "gemm_skinny" (1)      dedicated kernels for products with n <= 8 or k <= 8 */
 int cb200_tune(const char* key, int value);
 
 /* =====================================================================================================================
@@ -52,7 +52,7 @@ int cb200_tune(const char* key, int value);
 /* Marks [ptr, ptr+bytes) as L2-persisting for kernels subsequently launched on `stream` (stream access-policy window
  * + persisting-L2 carve-out).  Used for the top levels of the sum tree (the first 2^k entries of the heap array are
  * its top k levels), which every sample's descent re-reads while ~100 MB of minibatch traffic per step would
- * otherwise evict them from the 126 MB L2.  ptr == NULL clears the window.  CB200_ERR_UNSUPPORTED if the device has
+ * otherwise evict them from the 50 MB L2.  ptr == NULL clears the window.  CB200_ERR_UNSUPPORTED if the device has
  * no persisting-L2 support. */
 int cb200_l2_persist(const void* ptr, int64_t bytes, void* stream);
 
@@ -254,7 +254,7 @@ int cb200_gemm(const cb200_gemm_desc* h_desc, void* stream);
  *   mode 1: C[t * a_cols + c, :] = sum_q sum_b A[a_pix[t * num_q + q] * B + b, c] * G[q * B + b, :]   (weight gradient)
  * Replaces, for layers whose input already lives on the device as planes, the same reference code as cb200_gemm
  * (layers.py:108-183 forward, tf.gradients backward).  Operands move by 1-D bulk copies (TMA); 3xBF16 products with
- * fp32 TMEM accumulation, at most 32 reduction chunks of 32 per launch slice (use `splits`).
+ * fp32 accumulation (wgmma), at most 32 reduction chunks of 32 per launch slice (use `splits`).
  * ===================================================================================================================*/
 typedef struct cb200_tgemm_desc {
     int32_t mode;
@@ -296,7 +296,7 @@ typedef struct cb200_tgemm_desc {
     int32_t b_interleaved;      /* mode 0, n <= 64 (or n % 128 != 0): the B planes are "row-group interleaved" --        */
                                 /*   (row group | plane | column core | 64), written with plane_stride -1 by              */
                                 /*   cb200_split_planes (segment layout 1) / cb200_permute_f32 -- and the 3xBF16 product  */
-                                /*   set is issued as three wide tcgen05.mma on the [b1|b2|b3] operand                    */
+                                /*   set reads its three B planes from that one [b1|b2|b3] operand                         */
     const int32_t* a_pix_host;  /* mode 1, optional: HOST copy of a_pix.  When the taps that share a 128-row tile of the   */
                                 /*   result sit a constant number of pixels apart (at most three distinct strides over   */
                                 /*   the tiles: every convolution of the path), the A^T operand of a reduction chunk is  */

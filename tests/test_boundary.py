@@ -1,59 +1,39 @@
-"""The plug points of INTEGRATION.md checked against the UNMODIFIED reference (imported through oracle/ref_loader.py;
-skipped where /root/reference is absent, e.g. on the GPU box).  CPU only: nothing here launches a kernel -- the device
-classes are bound, resolved and type-checked, not run."""
+"""The plug points of INTEGRATION.md checked against what the UNMODIFIED reference exposes, recorded in
+tests/golden/boundary.json by oracle/make_golden_boundary.py: the argument lists of its memory methods and of the PER
+constructor, its Parameters defaults and its checkpoint-file conventions.  CPU only: nothing here launches a kernel --
+the device classes are bound, resolved and type-checked, not run."""
 import importlib
 import inspect
+import json
+import os
 
-import numpy as np
 import pytest
 
-from oracle import ref_loader
 
-needs_ref = pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present")
+@pytest.fixture
+def ref(golden_dir):
+    with open(os.path.join(golden_dir, "boundary.json")) as f:
+        return json.load(f)
 
 
-@needs_ref
-def test_bound_per_passes_the_reference_isinstance_gate_and_loader():
-    """INTEGRATION.md 'isinstance gates': a class derived from the device PER and the reference PER (device class first
-    in the MRO) satisfies ``isinstance(self.memory, PrioritizedExperienceReplay)``
-    (agents/value_optimization_agent.py:77) and is resolved by the reference's own
-    dynamic_import_and_instantiate_module_from_params (utils.py:389-404) from a Parameters.path string."""
-    ref_loader.load()
-    import rl_coach.memories.non_episodic.prioritized_experience_replay as ref
-    from rl_coach.agents.value_optimization_agent import ValueOptimizationAgent
-    from rl_coach.utils import short_dynamic_import
+def test_device_per_accepts_the_reference_constructor_and_resolves_from_its_path(ref):
+    """the device PER accepts every constructor argument of the reference PER, and its Parameters.path is the string the
+    reference's own loader (short_dynamic_import behind dynamic_import_and_instantiate_module_from_params,
+    utils.py:389-404) was recorded resolving to the device class; the project's resolver agrees"""
     from coach_b200.memories import prioritized_experience_replay as dev
-
-    class BoundPER(dev.PrioritizedExperienceReplay, ref.PrioritizedExperienceReplay):
-        def __init__(self, *args, **kwargs):
-            dev.PrioritizedExperienceReplay.__init__(self, *args, **kwargs)
-
-    # MRO: every public method the reference agents call comes from the device class
-    for name in ("store", "sample", "update_priorities", "num_transitions", "clean", "freeze", "get_transition"):
-        owner = next(c for c in BoundPER.__mro__ if name in c.__dict__)
-        assert owner.__module__.startswith("coach_b200"), (name, owner)
-    assert issubclass(BoundPER, ref.PrioritizedExperienceReplay)
-    # the gate of value_optimization_agent.py:77, evaluated by the reference's own code on an instance that was never
-    # constructed (no GPU here): isinstance only looks at the type
-    obj = BoundPER.__new__(BoundPER)
-    calls = []
-    from types import SimpleNamespace
-    fake = SimpleNamespace(memory=obj, call_memory=lambda f, a: calls.append(f))
-    batch = SimpleNamespace(info=lambda k: np.arange(3))
-    w = ValueOptimizationAgent.update_transition_priorities_and_get_weights(fake, [0.1, 0.2, 0.3], batch)
-    assert calls == ["update_priorities"] and w is not None
-    # the reference loader resolves the device class from its path string and passes the constructor arguments
+    from coach_b200.utils import short_dynamic_import
     params = dev.PrioritizedExperienceReplayParameters()
+    rec = ref["per_path_resolution"]
+    assert params.path == rec["path"]
+    assert rec["resolved"] == "coach_b200.memories.prioritized_experience_replay:PrioritizedExperienceReplay"
     cls = short_dynamic_import(params.path)
     assert cls is dev.PrioritizedExperienceReplay
     ctor = set(inspect.getfullargspec(cls).args)
-    ref_ctor = set(inspect.getfullargspec(ref.PrioritizedExperienceReplay).args)
-    assert ref_ctor <= ctor, "device PER must accept every constructor argument of the reference PER"
+    assert set(ref["per_constructor_args"]) <= ctor, "device PER must accept every constructor argument of the reference PER"
     passed = {k for k in params.__dict__ if k in ctor}
     assert {"max_size", "alpha", "beta", "epsilon", "allow_duplicates_in_batch_sampling"} <= passed
 
 
-@needs_ref
 @pytest.mark.parametrize("dev_path,ref_path,cls_name", [
     ("coach_b200.memories.experience_replay", "rl_coach.memories.non_episodic.experience_replay", "ExperienceReplay"),
     ("coach_b200.memories.prioritized_experience_replay", "rl_coach.memories.non_episodic.prioritized_experience_replay",
@@ -61,37 +41,28 @@ def test_bound_per_passes_the_reference_isinstance_gate_and_loader():
     ("coach_b200.memories.episodic_experience_replay", "rl_coach.memories.episodic.episodic_experience_replay",
      "EpisodicExperienceReplay"),
 ])
-def test_memory_method_surface_covers_the_reference(dev_path, ref_path, cls_name):
+def test_memory_method_surface_covers_the_reference(ref, dev_path, ref_path, cls_name):
     """every public method of the reference memory that the replay -> learn path calls exists on the device class with
     the same leading arguments"""
-    ref_loader.load()
+    assert ref["memory_modules"][cls_name] == ref_path, "golden data recorded from another reference class"
     dcls = getattr(importlib.import_module(dev_path), cls_name)
-    rcls = getattr(importlib.import_module(ref_path), cls_name)
     used = {"store", "sample", "num_transitions", "length", "clean", "freeze", "assert_not_frozen", "get_transition",
             "get", "remove_transition", "update_priorities", "store_episode", "num_complete_episodes",
             "num_transitions_in_complete_episodes", "verify_last_episode_is_closed", "mean_reward", "save",
             "load_pickled", "get_shuffled_training_data_generator"}
-    for name, fn in inspect.getmembers(rcls, inspect.isfunction):
+    methods = ref["memory_methods"][cls_name]
+    assert {"store", "sample", "num_transitions"} <= set(methods)
+    for name, ra in methods.items():
         if name not in used:
             continue
         assert hasattr(dcls, name), "%s.%s missing" % (cls_name, name)
-        ra = [a for a in inspect.getfullargspec(fn).args if a not in ("self", "lock")]
         da = [a for a in inspect.getfullargspec(getattr(dcls, name)).args if a not in ("self", "lock")]
         assert da[:len(ra)] == ra or name in ("sample",), (cls_name, name, ra, da)
 
 
-@needs_ref
-def test_parameter_defaults_match_the_reference():
+def test_parameter_defaults_match_the_reference(ref):
     """the Parameters classes carry the reference's defaults for every field they define (agents' algorithm / network
     parameters, memory parameters)"""
-    ref_loader.load()
-    from rl_coach.agents.dqn_agent import DQNAgentParameters as RDQN
-    from rl_coach.agents.ddqn_agent import DDQNAgentParameters as RDDQN
-    from rl_coach.agents.clipped_ppo_agent import ClippedPPOAgentParameters as RPPO
-    from rl_coach.agents.ddpg_agent import DDPGAgentParameters as RDDPG
-    from rl_coach.agents.td3_agent import TD3AgentParameters as RTD3
-    from rl_coach.agents.soft_actor_critic_agent import SoftActorCriticAgentParameters as RSAC
-    from rl_coach.agents.categorical_dqn_agent import CategoricalDQNAgentParameters as RC51
     from coach_b200.agents.categorical_dqn_agent import CategoricalDQNAgentParameters
     from coach_b200.agents.dqn_agent import DQNAgentParameters, DDQNAgentParameters
     from coach_b200.agents.clipped_ppo_agent import ClippedPPOAgentParameters
@@ -99,32 +70,33 @@ def test_parameter_defaults_match_the_reference():
     from coach_b200.agents.soft_actor_critic_agent import SoftActorCriticAgentParameters
 
     def same(a, b):
-        if hasattr(a, "num_steps"):
-            return type(a).__name__ == type(b).__name__ and a.num_steps == b.num_steps
-        if hasattr(a, "current_value"):
-            return float(a.current_value) == float(b.current_value)
-        if hasattr(b, "name") and isinstance(a, str):      # enums of the reference are plain strings here
-            return a == b.name
-        if isinstance(a, (int, float, str, bool, type(None), tuple)):
-            return a == b
-        return True                                   # structured values (filters, lists of layer objects): not compared
+        if b is None:
+            return True                               # structured values (filters, lists of layer objects): not compared
+        if "num_steps" in b:
+            return type(a).__name__ == b["steps_type"] and a.num_steps == b["num_steps"]
+        if "schedule_value" in b:
+            return float(a.current_value) == b["schedule_value"]
+        if "enum" in b:                               # enums of the reference are plain strings here
+            return a == b["enum"] or getattr(a, "name", None) == b["enum"]
+        if "tuple" in b:
+            return tuple(a) == tuple(b["tuple"])
+        return a == b["value"]
 
     own_only = {"hidden_units", "truncate_dataset_to_playing_steps", "middleware_parameters", "heads_parameters"}
-    for mine, ref in ((DQNAgentParameters(), RDQN()), (DDQNAgentParameters(), RDDQN()),
-                      (ClippedPPOAgentParameters(), RPPO()), (DDPGAgentParameters(), RDDPG()),
-                      (TD3AgentParameters(), RTD3()), (SoftActorCriticAgentParameters(), RSAC()),
-                      (CategoricalDQNAgentParameters(), RC51())):
+    for mine in (DQNAgentParameters(), DDQNAgentParameters(), ClippedPPOAgentParameters(), DDPGAgentParameters(),
+                 TD3AgentParameters(), SoftActorCriticAgentParameters(), CategoricalDQNAgentParameters()):
+        r = ref["parameters"][type(mine).__name__]
         for k, v in vars(mine.algorithm).items():
-            if k in own_only or not hasattr(ref.algorithm, k):
+            if k in own_only or k not in r["algorithm"]:
                 continue
-            assert same(v, getattr(ref.algorithm, k)), (type(mine).__name__, "algorithm", k, v, getattr(ref.algorithm, k))
+            assert same(v, r["algorithm"][k]), (type(mine).__name__, "algorithm", k, v, r["algorithm"][k])
         for net in mine.network_wrappers:
             for k, v in vars(mine.network_wrappers[net]).items():
-                if k in own_only or not hasattr(ref.network_wrappers[net], k):
+                if k in own_only or k not in r["network_wrappers"][net]:
                     continue
-                rv = getattr(ref.network_wrappers[net], k)
+                rv = r["network_wrappers"][net][k]
                 assert same(v, rv), (type(mine).__name__, net, k, v, rv)
-        assert type(mine.memory).__name__ == type(ref.memory).__name__, type(mine).__name__
+        assert type(mine.memory).__name__ == r["memory_class"], type(mine).__name__
 
 
 def test_presets_define_the_five_baseline_configurations():
@@ -145,30 +117,24 @@ def test_presets_define_the_five_baseline_configurations():
     assert qn.store.num_params() - 1 == 3293863          # SURVEY section 8d, config 5 (+1: the rescaler scalar)
 
 
-@needs_ref
-def test_checkpoint_names_and_state_file_interoperate_with_the_reference(tmp_path):
+def test_checkpoint_names_and_state_file_interoperate_with_the_reference(ref, tmp_path):
     """coach_b200/checkpoint.py follows the reference's on-disk conventions (checkpoint.py:115-155, :247-273,
-    graph_manager.py:630): the reference's CheckpointStateFile / CheckpointFilenameParser read what we write -- number
-    and name -- and we read what the reference writes; a half-written or foreign state file is ignored by both."""
-    ref_loader.load()
-    from rl_coach.checkpoint import (CheckpointFilenameParser, CheckpointStateFile, CheckpointStateReader,
-                                     SingleCheckpoint)
+    graph_manager.py:630): the state file has the reference's name and the content its CheckpointStateFile writes, we
+    read what the reference writes, and a half-written or foreign state file yields no checkpoint."""
     from coach_b200 import checkpoint as ck
     d = str(tmp_path)
     name = ck.checkpoint_name(7, 123456)
     assert name == "7_Step-123456.ckpt"                                   # '{}_Step-{}.ckpt' of graph_manager.py:630
-    parsed = CheckpointFilenameParser().parse(name)
-    assert parsed is not None and parsed.num == 7 and parsed.name == name
-    ck._write_state_file(d, name)
-    assert CheckpointStateFile.checkpoint_state_filename == ck.STATE_FILE
-    got = CheckpointStateFile(d).read()
-    assert got == SingleCheckpoint(7, name)
-    assert CheckpointStateReader(d, checkpoint_state_optional=False).get_latest() == SingleCheckpoint(7, name)
-    # the other direction
-    CheckpointStateFile(d).write(SingleCheckpoint(12, ck.checkpoint_name(12, 99)))
+    sf = ref["checkpoint_state_file"]
+    assert ck.STATE_FILE == sf["name"]
+    # what the reference's CheckpointStateFile(d).write(SingleCheckpoint(12, "12_Step-99.ckpt")) leaves on disk
+    ck._write_state_file(d, ck.checkpoint_name(12, 99))
+    with open(os.path.join(d, ck.STATE_FILE)) as f:
+        assert f.read() == sf["content_for_12_Step-99"]
+    with open(os.path.join(d, ck.STATE_FILE), "w") as f:
+        f.write(sf["content_for_12_Step-99"])
     assert ck.read_state_file(d) == "12_Step-99.ckpt"
-    # garbage in the state file: no checkpoint for either reader
-    with open(str(tmp_path / ck.STATE_FILE), "w") as f:
+    # garbage in the state file: no checkpoint
+    with open(os.path.join(d, ck.STATE_FILE), "w") as f:
         f.write("not a checkpoint")
     assert ck.read_state_file(d) is None
-    assert CheckpointStateFile(d).read() is None

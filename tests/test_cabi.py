@@ -1,4 +1,4 @@
-"""CPU-only checks of the C-ABI boundary: the library builds for sm_100a, loads, and exports every symbol that
+"""CPU-only checks of the C-ABI boundary: the library builds for sm_90a, loads, and exports every symbol that
 include/coach_b200.h declares; the ctypes table in coach_b200/_lib.py covers the same set.  No compute calls."""
 import os
 import re
@@ -30,12 +30,12 @@ def test_ctypes_table_matches_header():
     assert sorted(_lib.PROTOTYPES.keys()) == header_symbols()
 
 
-def test_only_sm100a_code_in_library():
+def test_only_sm90a_code_in_library():
     import subprocess
     from coach_b200 import build
     out = subprocess.run(["cuobjdump", "-lelf", build.build()], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_argument_errors_surface_as_valueerror():
@@ -101,3 +101,12 @@ def test_plane_format_helpers_roundtrip():
     assert tl.channels_ok(64) and tl.channels_ok(256) and not tl.channels_ok(48) and not tl.channels_ok(192 + 8)
     assert tl.width_ok(32) and tl.width_ok(512) and not tl.width_ok(16) and not tl.width_ok(96)
     assert tl.pick_splits_tiled(4, 1296) >= 41          # at most 32 chunks per slice
+
+
+def test_removed_tune_key_is_rejected():
+    # "gemm_persistent" selected a schedule that no longer exists: an error, not a silently ignored switch
+    from coach_b200 import _lib
+    lib = _lib.load()
+    assert lib.cb200_tune(b"gemm_persistent", 1) == -1
+    assert b"gemm_persistent" in lib.cb200_last_error()
+    assert lib.cb200_tune(b"gemm_tc", 1) == 0

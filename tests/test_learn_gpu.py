@@ -453,47 +453,6 @@ def test_dqn_graph_replay_matches_eager(monkeypatch):
     assert torch.equal(results[0][2], results[1][2])
 
 
-def test_persistent_schedule_is_bit_identical():
-    """cb200_tune("gemm_persistent", 1): the persistent tiled GEMM (epilogue of unit i under the main loop of unit
-    i+1, two TMEM accumulator sets) computes every unit with the same operation order -> identical bits"""
-    from coach_b200.architectures import tiled as tl
-    from coach_b200.architectures.layers import Conv2d, Workspace
-    L, lib = _lib()
-    dev = torch.device("cuda")
-    B, H, C, N, K, S = 160, 20, 32, 64, 4, 2
-    g = torch.Generator().manual_seed(11)
-    layer0 = Conv2d((H, H), C, N, K, S, "relu")
-    OH = layer0.OH
-    x = torch.relu(torch.randn(B, H, H, C, generator=g)).to(dev)
-    w = (torch.randn(K, K, C, N, generator=g) / np.sqrt(K * K * C)).to(dev)
-    b = (torch.randn(N, generator=g) * 0.1).to(dev)
-    dy = torch.randn(B, OH, OH, N, generator=g).to(dev)
-    outs = []
-    try:
-        for persistent in (0, 1):
-            lib.cb200_tune(b"gemm_persistent", persistent)
-            layer = Conv2d((H, H), C, N, K, S, "relu")
-            y = torch.empty(B, OH * OH * N, device=dev)
-            flat = torch.empty(K * K * C * N + N, device=dev)
-            dw, db = flat[:K * K * C * N].view(K, K, C, N), flat[K * K * C * N:]
-            dx = torch.empty(B, H * H * C, device=dev)
-            ws = Workspace(dev)
-            wp = tl.PlaneBuf(K * K * C, N, dev, interleaved=tl.b_interleaved(N)).load(lib, w)
-            ctx = tl.PlaneCtx(x=tl.PlaneBuf(H * H * B, C, dev, npix=H * H).load(lib, _pixel_major(x, B, H * H, C)),
-                              y=tl.PlaneBuf(OH * OH * B, N, dev, npix=OH * OH),
-                              dy=tl.PlaneBuf(OH * OH * B, N, dev, npix=OH * OH).load(lib, _pixel_major(dy, B, OH * OH, N)),
-                              dx=tl.PlaneBuf(H * H * B, C, dev, npix=H * H), w_ptr=wp.ptr, w_stride=wp.stride)
-            layer.prepare(lib, ws, B, dev, x, y, w, b, dw, db, dy, dx, need_dx=True, prev_act=1, planes=ctx)
-            layer.forward()
-            layer.backward()
-            torch.cuda.synchronize()
-            outs.append((y.clone(), flat.clone(), dx.clone(), ctx.y.t.clone(), ctx.dx.t.clone()))
-    finally:
-        lib.cb200_tune(b"gemm_persistent", 0)
-    for a, c in zip(outs[0], outs[1]):
-        assert torch.equal(a, c)
-
-
 @pytest.mark.parametrize("E", [16, 128])
 def test_acting_path_batched_q_values_and_e_greedy(E):
     """DQNAgent.choose_actions: the batched online-network forward equals the oracle's Q-values and the actions are the

@@ -18,7 +18,7 @@ def timed(fn, flush, iters=30, warmup=5):
         fn()
     ts = []
     for _ in range(iters):
-        flush.fill_(1)                       # evict L2 (126 MB) with a 256 MB write
+        flush.fill_(1)                       # evict L2 (50 MB) with a 256 MB write
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         s.record()
         fn()
