@@ -72,6 +72,7 @@ class Column(ctypes.Structure):
 PROTOTYPES = {
     "cb200_abi_version": (c_int, []),
     "cb200_last_error": (ctypes.c_char_p, []),
+    "cb200_last_dispatch": (ctypes.c_char_p, []),
     "cb200_launch_count": (c_i64, []),
     "cb200_device_info": (c_int, [ctypes.POINTER(c_int)] * 3),
     "cb200_tune": (c_int, [ctypes.c_char_p, c_int]),

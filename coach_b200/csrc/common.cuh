@@ -41,6 +41,11 @@ void set_error(const char* fmt, ...);
 
 static inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// what cb200_last_dispatch() reports: the kernel the calling thread's last GEMM call launched (a static string), the
+// A^T fetch mode of a weight-gradient call (or NULL) and the split-reduction kernel (reset by set_dispatch)
+void set_dispatch(const char* kernel, const char* fetch = nullptr);
+void set_dispatch_reduce(const char* reduce);
+
 int sm_count();   // cached multiprocessor count of the current device
 int tune_get(const char* key, int dflt, int lo, int hi);   // runtime knob set through cb200_tune()
 

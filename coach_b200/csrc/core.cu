@@ -25,6 +25,19 @@ void set_error(const char* fmt, ...) {
 
 void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
+// cb200_last_dispatch: the GEMM entry points store static names here, the string is only assembled when asked for
+static thread_local const char* g_dispatch_kernel = "";
+static thread_local const char* g_dispatch_fetch = nullptr;
+static thread_local const char* g_dispatch_reduce = nullptr;
+static thread_local char g_dispatch[128] = "";
+
+void set_dispatch(const char* kernel, const char* fetch) {
+    g_dispatch_kernel = kernel;
+    g_dispatch_fetch = fetch;
+    g_dispatch_reduce = nullptr;
+}
+void set_dispatch_reduce(const char* reduce) { g_dispatch_reduce = reduce; }
+
 int sm_count() {
     static int cached[64] = {0};
     int dev = 0;
@@ -53,6 +66,12 @@ extern "C" {
 
 int cb200_abi_version(void) { return CB200_ABI_VERSION; }
 const char* cb200_last_error(void) { return cb200::g_error; }
+const char* cb200_last_dispatch(void) {
+    snprintf(cb200::g_dispatch, sizeof(cb200::g_dispatch), "%s%s%s%s%s", cb200::g_dispatch_kernel,
+             cb200::g_dispatch_fetch ? "/" : "", cb200::g_dispatch_fetch ? cb200::g_dispatch_fetch : "",
+             cb200::g_dispatch_reduce ? "+" : "", cb200::g_dispatch_reduce ? cb200::g_dispatch_reduce : "");
+    return cb200::g_dispatch;
+}
 int64_t cb200_launch_count(void) { return cb200::g_launches.load(std::memory_order_relaxed); }
 
 int cb200_tune(const char* key, int value) {

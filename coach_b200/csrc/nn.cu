@@ -1,9 +1,19 @@
 // coach_b200/csrc/nn.cu -- C-ABI entry points of the dense contractions of the learn step (see nn_gemm.cuh).
+#include <string>
+
 #include "nn_gemm_skinny.cuh"
 #include "nn_gemm_tiled.cuh"
 
 namespace cb200 {
 namespace gemm {
+
+// kernel names for cb200_last_dispatch, built once per template instantiation
+static std::string kernel_name(const char* kind, int a, int b, const char* c, const char* d = nullptr) {
+    char s[64];
+    if (b > 0) snprintf(s, sizeof(s), "%s<%d,%d,%s%s%s>", kind, a, b, c, d ? "," : "", d ? d : "");
+    else snprintf(s, sizeof(s), "%s<%d,%s%s%s>", kind, a, c, d ? "," : "", d ? d : "");
+    return s;
+}
 
 using CfgN64 = Cfg<128, 64, 16, 8, 8>;   // 128 threads, 8x8 per thread
 using CfgN32 = Cfg<128, 32, 16, 8, 4>;   // 128 threads, 8x4 per thread
@@ -34,6 +44,8 @@ static void launch(const cb200_gemm_desc& d, int M, int R, int splits, int r_per
     bl.N = d.n;
     bl.ldb = d.ldb;
     const EpiParams ep = make_epi(d, splits);
+    static const std::string name = kernel_name("ffma", C::BM, C::BN, kT ? "T" : "N");
+    set_dispatch(name.c_str());
     dim3 grid((M + C::BM - 1) / C::BM, (d.n + C::BN - 1) / C::BN, splits);
     gemm_kernel<C, kT><<<grid, C::T, 0, st>>>(al, bl, ep, M, d.n, R, r_per_split);
     count_launch();
@@ -58,6 +70,8 @@ static void launch_fast(const cb200_gemm_desc& d, int M, int R, int splits, int 
     a.cols = d.a_cols;
     a.ones_col = (kT && d.a_ones_col) ? d.a_cols : -1;
     const EpiParams ep = make_epi(d, splits);
+    static const std::string name = kernel_name("fast", C::BM, C::BN, kT ? "T" : "N");
+    set_dispatch(name.c_str());
     dim3 grid((M + C::BM - 1) / C::BM, (d.n + C::BN - 1) / C::BN, splits);
     gemm_fast_kernel<C, kT><<<grid, C::T, 0, st>>>(a, d.b, d.ldb, ep, M, d.n, R, r_per_split);
     count_launch();
@@ -90,6 +104,9 @@ static int launch_tc(const cb200_gemm_desc& d, int M, int R, int splits, int r_p
             return -1;
         configured = true;
     }
+    static const std::string names[2] = {kernel_name("tc", BN, 0, kT ? "T" : "N", kU8 ? "u8" : "f32"),
+                                         kernel_name("tc", BN, 0, kT ? "T" : "N", "lut")};
+    set_dispatch(names[!kU8 && d.a_lut ? 1 : 0].c_str());
     dim3 grid((M + kTcBM - 1) / kTcBM, (d.n + BN - 1) / BN, splits);
     const bool bp = d.b_planes != nullptr && d.n % 8 == 0 && d.ldb == d.n && R % 8 == 0;
     gemm_tc_kernel<BN, kT, kU8><<<grid, 128, smem, st>>>(a, d.b, d.ldb, ep, M, d.n, R, r_per_split, d.a_u8_div,
@@ -174,6 +191,10 @@ static int launch_tiled(const CUtensorMap* maps, const TiledParams& tp, const Ep
             return -1;
         configured = true;
     }
+    static const std::string name = kernel_name("tiled", BN, 0, kT ? "T" : "N",
+                                                NA == 1 ? (kCat ? "1,cat" : "1") : (kCat ? "3,cat" : "3"));
+    static const char* const fetch[4] = {"bulk", "tma1", "tma2", "tma3"};
+    set_dispatch(name.c_str(), kT ? fetch[tp.a_tma] : nullptr);
     dim3 grid(gx, (tp.n + BN - 1) / BN, splits);
     // maps: [0] A (mode 0) / A^T class 0 (mode 1), [1] B, [2], [3] A^T classes 1 and 2
     gemm_tc_tiled_kernel<BN, kT, NA, kCat><<<grid, kTlThreads, smem, st>>>(maps[0], maps[1], maps[2], maps[3], tp, ep, M);
@@ -351,7 +372,6 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
     const int R = tr ? d->a_rows : d->a_cols;
     int splits = d->splits > 1 ? d->splits : 1;
     CB200_CHECK_ARG(splits == 1 || d->workspace, "split reduction needs a workspace");
-    CB200_CHECK_ARG(splits == 1 || !d->accumulate || true, "");
     int r_per_split = (R + splits - 1) / splits;
     r_per_split = (r_per_split + 15) / 16 * 16;
     splits = (R + r_per_split - 1) / r_per_split;
@@ -362,6 +382,7 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
         const bool al16 = (reinterpret_cast<uintptr_t>(a) & 15) == 0 && d->a_lda % 4 == 0;
         const gemm::EpiParams ep = gemm::make_epi(*d, 1);
         if (!tr && d->n <= 8 && R % 4 == 0 && al16) {
+            set_dispatch("skinny_n");
             gemm::skinny_n_kernel<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(a, d->a_lda, d->b, d->ldb, ep, M, d->n, R);
             count_launch();
             CB200_CHECK_LAUNCH();
@@ -369,6 +390,7 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
         }
         if (!tr && R <= 8 && d->n % 4 == 0 && d->ldb % 4 == 0 && (reinterpret_cast<uintptr_t>(d->b) & 15) == 0) {
             const int64_t groups = (int64_t)M * (d->n / 4);
+            set_dispatch("skinny_r");
             gemm::skinny_r_kernel<<<(unsigned)((groups + 255) / 256), 256, 0, st>>>(a, d->a_lda, d->b, d->ldb, ep, M,
                                                                                      d->n, R);
             count_launch();
@@ -377,6 +399,7 @@ int cb200_gemm(const cb200_gemm_desc* d, void* stream) {
         }
         if (tr && d->n <= 8) {
             const int kblocks = (d->a_cols + 31) / 32;
+            set_dispatch("skinny_tn");
             gemm::skinny_tn_kernel<<<(unsigned)(kblocks + (ones ? 1 : 0)), 1024, 0, st>>>(
                 a, d->a_lda, d->b, d->ldb, ep, d->a_rows, d->a_cols, d->n, d->a_cols);
             count_launch();
@@ -476,8 +499,8 @@ int cb200_gemm_tiled(const cb200_tgemm_desc* d, void* stream) {
     const int bn = d->n <= 32 ? 32 : ((d->n <= 64 || d->n % 128 != 0) ? 64 : 128);
     const int na = d->a_num_planes == 1 ? 1 : 3;
     CB200_CHECK_ARG(na == 3 || d->a_u8_div > 0.f, "a single A plane means raw uint8 values: a_u8_div must be set");
-    // row-group interleaved B planes: the three B planes reach shared memory as one [32 k, 3 n] operand and the 3xBF16
-    // product set is issued as 3 wide MMAs instead of 6 (half the shared-memory operand reads of the tensor pipe)
+    // row-group interleaved B planes: the three B planes reach shared memory as one [32 k, 3 n] operand (one TMA box
+    // instead of three); the 3xBF16 product set is still issued as six narrow MMAs, one per plane pair
     const bool cat = d->b_interleaved != 0;
     CB200_CHECK_ARG(!cat || (d->mode == 0 && bn <= 64), "b_interleaved needs mode 0 and n <= 64 (or n % 128 != 0)");
     // the tensor maps depend only on the descriptor: built on the first call, kept in the descriptor

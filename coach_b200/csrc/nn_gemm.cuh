@@ -352,10 +352,13 @@ __global__ void __launch_bounds__(256) split_reduce_wide_kernel(EpiParams ep, in
 inline void launch_split_reduce(const EpiParams& ep, int M, int N, cudaStream_t st) {
     const int64_t total = (int64_t)M * N;
     if (ep.splits >= 16 && total <= (1 << 16)) {
+        set_dispatch_reduce("reduce_wide");
         split_reduce_wide_kernel<<<(unsigned)((total + 31) / 32), 256, 0, st>>>(ep, M, N);
     } else if (N % 4 == 0 && total % 4 == 0 && (reinterpret_cast<uintptr_t>(ep.partial) & 15) == 0) {
+        set_dispatch_reduce("reduce_vec");
         split_reduce_kernel<true><<<(unsigned)((total / 4 + 255) / 256), 256, 0, st>>>(ep, M, N);
     } else {
+        set_dispatch_reduce("reduce_scalar");
         split_reduce_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ep, M, N);
     }
 }

@@ -32,6 +32,12 @@ extern "C" {
 
 int cb200_abi_version(void);
 const char* cb200_last_error(void);
+/* Thread-local name of the kernel the calling thread's last cb200_gemm / cb200_gemm_tiled call launched, e.g.
+ * "tc<64,T,u8>+reduce_wide", "tiled<64,N,3,cat>", "tiled<128,T,3>/tma2", "ffma<32,32,N>", "skinny_n": the kernel
+ * (template width(s), N / T = plain / transposed A, operand kind or A planes), "/fetch" of a mode-1 tiled call (bulk,
+ * tma1 .. tma3 = number of A^T tensor-map classes) and "+reduce_wide|vec|scalar" when a split reduction followed.
+ * Lets tests prove which variants they ran; valid until the thread's next call of this function. */
+const char* cb200_last_dispatch(void);
 /* Number of kernels launched through this library by the calling process so far (bench.py's `gpu_launches`). */
 int64_t cb200_launch_count(void);
 /* Multiprocessor count and compute capability of the current device (any pointer may be NULL). */
@@ -220,7 +226,8 @@ typedef struct cb200_gemm_desc {
     int32_t splits;             /* 0 / 1 = no split; k > 1 = k partial sums reduced in fixed order                   */
     /* fast-path hints (the tables are built by the caller, who knows their structure) */
     int32_t a_vec4;             /* 1: every aligned group of 4 column indices is contiguous in memory, a_cols % 4 == 0 */
-                                /*    and every a_rowoff % 4 == 0  => 128-bit (fp32) / 32-bit (uint8) operand loads   */
+                                /*    and every a_rowoff % 4 == 0  => 128-bit (fp32) / 32-bit (uint8) operand loads;  */
+                                /*    a_colinfo must then be equal within each such group (the mask is per group)     */
     int32_t a_ones_col;         /* a_transposed only: 1 = append an output row a_cols holding sum_m B[m, :] (the bias  */
                                 /*    gradient lands in c[a_cols, :], i.e. right behind the kernel gradient)          */
     float a_u8_div;             /* uint8 A only, 0 = not declared: the caller states a_lut[v] == (float)v / a_u8_div.  */

@@ -9,6 +9,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+import gemm_ref as gr
 from coach_b200 import _lib
 from coach_b200.architectures import tiled as tl
 from coach_b200.architectures.layers import Conv2d, Dense, Workspace
@@ -22,14 +23,11 @@ def _tensor_at(op, ptr):
 
 
 def _mode0(op, A, W_blocks, B):
-    """C[q*B+b, :] = sum_{(a_pix, w_blk) in list(q)} A[a_pix*B+b, :] @ W[w_blk]   (A: [pix*B, Ca], W: [blocks, Ca, n])"""
+    """mode-0 contraction (gemm_ref.tiled_mode0) with the tap lists of a prepared call"""
     d = op.desc
     ptr = _tensor_at(op, d.list_ptr).numpy()
     lst = _tensor_at(op, d.list).numpy().reshape(-1, 2)
-    out = np.zeros((d.num_q * B, d.n))
-    for q in range(d.num_q):
-        for a_pix, w_blk in lst[ptr[q]:ptr[q + 1]]:
-            out[q * B:(q + 1) * B] += A[a_pix * B:(a_pix + 1) * B] @ W_blocks[w_blk]
+    out = gr.tiled_mode0(ptr, lst, A, W_blocks, B, d.num_q, d.n)
     if d.c_rowmap:
         rm = _tensor_at(op, d.c_rowmap).numpy()
         res = np.zeros_like(out)
@@ -39,14 +37,9 @@ def _mode0(op, A, W_blocks, B):
 
 
 def _mode1(op, A, G, B):
-    """C[t*Ca+c, :] = sum_q sum_b A[a_pix[t, q]*B+b, c] * G[q*B+b, :]"""
+    """mode-1 contraction (gemm_ref.tiled_mode1) with the pixel table of a prepared call"""
     d = op.desc
-    apix = _tensor_at(op, d.a_pix).numpy().reshape(d.taps, d.num_q)
-    Ca = d.a_cols
-    out = np.zeros((d.taps * Ca, d.n))
-    for t in range(d.taps):
-        for q in range(d.num_q):
-            out[t * Ca:(t + 1) * Ca] += A[apix[t, q] * B:(apix[t, q] + 1) * B].T @ G[q * B:(q + 1) * B]
+    out = gr.tiled_mode1(_tensor_at(op, d.a_pix).numpy(), A, G, B, d.taps, d.num_q)
     if d.c_rowmap:
         rm = _tensor_at(op, d.c_rowmap).numpy()
         res = np.zeros((int(rm.max()) + 1, d.n))
