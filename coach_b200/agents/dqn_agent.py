@@ -87,16 +87,25 @@ class QNetworkWrapper(object):
         self.target_s2 = net_def.instantiate(lib, self.ws_target, batch_size, s2, self.theta_target) \
             if self.theta_target is not None else None
         self.online_s2 = net_def.instantiate(lib, self.ws, batch_size, s2, self.theta) if double_dqn else None
-        # Adam state: fp32 running powers exactly like TF's non-slot beta1_power / beta2_power variables
-        self.beta1_power = np.float32(params.adam_optimizer_beta1)
-        self.beta2_power = np.float32(params.adam_optimizer_beta2)
         self.sumsq = torch.zeros(1, dtype=torch.float32, device=device)
         self.has_target = self.theta_target is not None
-        # device copy of the running powers: the optimizer step then has constant launch parameters and the whole
-        # learn step can be captured in a CUDA graph (cb200_adam_tf_dev)
+        # Adam state: the fp32 running powers of TF's non-slot beta1 / beta2 power variables, kept on the device
+        # so that the optimizer step has constant launch parameters and can be captured in a CUDA graph
+        # (cb200_adam_tf_dev)
         self.adam_state = torch.tensor([params.adam_optimizer_beta1, params.adam_optimizer_beta2],
                                        dtype=torch.float32, device=device)
-        self.device_adam_state = False
+        # parameter planes (operands of the tensor-core GEMMs) are re-derived where the parameters are written, not in
+        # every forward pass: the target network's once per target update instead of once per learn step
+        self._planes = []
+        for inst in (self.online_s, self.online_s2, self.target_s2):
+            self.add_planes(inst)
+
+    def add_planes(self, inst):
+        """derives the operand planes of ``inst`` (a network instance over theta or theta_target) now and again
+        whenever those parameters change"""
+        if inst is not None and inst.theta_planes is not None:
+            self._planes.append(inst.theta_planes)
+            inst.theta_planes.refresh()
 
     def sync(self):
         """online -> target hard copy (network_wrapper.py:94-107)."""
@@ -107,20 +116,9 @@ class QNetworkWrapper(object):
                                          float(rate), _lib.current_stream()))
         self.target_changed()
 
-    # ---- parameter planes (operands of the tensor-core GEMMs) are re-derived where the parameters are written, not in
-    # every forward pass: the target network's once per target update instead of once per learn step -----------------
-    def manage_planes(self):
-        self._managed = [i for i in (self.online_s, self.online_s2, self.target_s2) if i is not None and
-                         i.manage_planes()]
-        self.online_changed()
-        self.target_changed()
-
     def _refresh(self, theta):
-        done = set()
-        for inst in getattr(self, "_managed", ()):
-            tp = inst.theta_planes
-            if tp.theta.data_ptr() == theta.data_ptr() and id(tp) not in done:
-                done.add(id(tp))
+        for tp in self._planes:
+            if tp.theta.data_ptr() == theta.data_ptr():
                 tp.refresh()
 
     def online_changed(self):
@@ -132,32 +130,21 @@ class QNetworkWrapper(object):
         if self.theta_target is not None:
             self._refresh(self.theta_target)
 
-    def apply_gradients(self, scaler=1.0, grad=None):
+    def apply_gradients(self, scaler=1.0):
         """clip is applied by the caller (accumulate_gradients side in the reference); here: optional rescale,
-        then the optimizer (architecture.py:469-521).  grad: flat gradient buffer to apply (default: store.grad)."""
+        then the optimizer (architecture.py:469-521)."""
         st = _lib.current_stream()
         n = self.store.size
-        grad = self.store.grad if grad is None else grad
+        grad = self.store.grad
         if scaler != 1.0:
             _lib.check(self.lib.cb200_scale(grad.data_ptr(), n, float(scaler), st))
         p = self.params
         if p.optimizer_type != 'Adam':
             raise NotImplementedError("only the Adam optimizer of the DQN presets is implemented on device")
-        if self.device_adam_state:
-            _lib.check(self.lib.cb200_adam_tf_dev(self.theta.data_ptr(), self.store.m.data_ptr(),
-                                                  self.store.v.data_ptr(), grad.data_ptr(), n,
-                                                  float(p.learning_rate), float(p.adam_optimizer_beta1),
-                                                  float(p.adam_optimizer_beta2), float(p.optimizer_epsilon),
-                                                  self.adam_state.data_ptr(), st))
-            self.online_changed()
-            return
-        _lib.check(self.lib.cb200_adam_tf(self.theta.data_ptr(), self.store.m.data_ptr(), self.store.v.data_ptr(),
-                                          grad.data_ptr(), n, float(p.learning_rate),
-                                          float(p.adam_optimizer_beta1), float(p.adam_optimizer_beta2),
-                                          float(p.optimizer_epsilon), float(self.beta1_power),
-                                          float(self.beta2_power), st))
-        self.beta1_power = np.float32(self.beta1_power * np.float32(p.adam_optimizer_beta1))
-        self.beta2_power = np.float32(self.beta2_power * np.float32(p.adam_optimizer_beta2))
+        _lib.check(self.lib.cb200_adam_tf_dev(self.theta.data_ptr(), self.store.m.data_ptr(), self.store.v.data_ptr(),
+                                              grad.data_ptr(), n, float(p.learning_rate),
+                                              float(p.adam_optimizer_beta1), float(p.adam_optimizer_beta2),
+                                              float(p.optimizer_epsilon), self.adam_state.data_ptr(), st))
         self.online_changed()
 
 
@@ -222,8 +209,6 @@ class DQNAgent(object):
                                                  input_planes=self.s2d["columns"] if self.s2d else None)}
         if self.networks["main"].has_target:
             self.networks["main"].sync()
-        if _lib.tune_default("managed_planes", 1):
-            self.networks["main"].manage_planes()
         # plain Q head: head forward passes, TD targets, loss and the head's backward pass are ONE fused launch
         net = self.networks["main"]
         self.head_desc = None
@@ -242,33 +227,26 @@ class DQNAgent(object):
         self._pr_dev = torch.zeros(B, dtype=torch.float64, device=dev)
         self._fetch_host = torch.zeros(2, dtype=torch.float32, pin_memory=pin)
         self._loss_host = torch.zeros(1, dtype=torch.float32, pin_memory=pin)    # loss of the forward part (fused head)
-        # CUDA graphs of the learn step (own minibatch buffers only): forward + TD targets | loss + backward + clip
-        # [+ Adam when there is no all-reduce in between].  Every launch parameter of those kernels is constant from
-        # step to step, so two graph launches replace ~45 kernel launches; the first steps run eagerly (they build
-        # the TMA tensor maps, size the workspace and configure shared memory).
+        # CUDA graphs of the learn step (own minibatch buffers only), one per part: forward + TD targets | loss +
+        # backward [+ norm + clip] | [norm +] Adam + plane refresh.  Every launch parameter of those kernels is constant
+        # from step to step, so three graph launches replace ~45 kernel launches; the first steps run eagerly (they
+        # build the TMA tensor maps, size the workspace and configure shared memory).
         self.use_graph = bool(_lib.tune_default("dqn_graph", 1)) and dev.type == "cuda" and B >= 128
-        self.networks["main"].device_adam_state = self.use_graph
         # two more CUDA streams per learn step: the target network's forward pass runs beside the online network's, the
         # weight-gradient GEMMs beside the data-gradient chain (layers.SideStream; parallel branches of the CUDA graphs)
-        streams = bool(_lib.tune_default("dqn_streams", 1)) and dev.type == "cuda"
-        self._side_fwd = SideStream(dev) if streams else NO_SIDE
-        self._side_w = SideStream(dev) if streams else NO_SIDE
+        self._side_fwd = SideStream(dev)
+        self._side_w = SideStream(dev)
         # the tree update of a step only needs the TD errors of its forward part: it runs beside the backward pass and
         # the optimizer; the next sample waits for it (sample_batch)
-        self._side_upd = SideStream(dev) if streams else NO_SIDE
-        # ... and the optimizer part of a step ([all-reduce,] Adam, plane refresh) runs on a fourth stream: the next
-        # step's sample + gather does not depend on it and starts as soon as the backward pass is done
-        self._side_opt = SideStream(dev) if streams and _lib.tune_default("dqn_opt_stream", 1) else NO_SIDE
-        if streams and isinstance(self.memory, PrioritizedExperienceReplay):
+        self._side_upd = SideStream(dev)
+        # ... and the optimizer part of a replayed step (Adam, plane refresh) runs on a fourth stream: the next step's
+        # sample + gather does not depend on it and starts as soon as the backward pass (and the all-reduce) is done
+        self._side_opt = SideStream(dev)
+        if isinstance(self.memory, PrioritizedExperienceReplay):
             self.memory._update_side = self._side_upd          # every other tree access of the memory joins it first
-        self._graphs = None
+        self._graphs = None                       # [(graph, kernels in it)] of the three parts, once captured
         self._acting = {}                         # number of environments -> (input buffer, forward-only online network)
-        self._graph_c = (None, 0)
-        self._collectives_in_graph = False
-        self._opt_on_stream = False
-        self._early_loss = bool(_lib.tune_default("dqn_early_loss", 1))
-        self._head_weights, self._head_split = None, False
-        self._grad_sync = None                    # exchange buffer of the overlapped gradient all-reduce
+        self._head_weights = None
         self._eager_steps = 0
         self.graph_kernel_launches = 0            # kernels executed through graph replays (bench.py gpu_launches)
         # counters of agents/agent.py:112-135
@@ -355,9 +333,7 @@ class DQNAgent(object):
                               device=self.device)
             # (own workspace: growing the learn step's would invalidate the pointers baked into its CUDA graphs)
             on = self.net_def.instantiate(self.lib, Workspace(self.device), E, buf, net.theta)
-            if getattr(net, "_managed", None) is not None and on.manage_planes():
-                net._managed.append(on)
-                on.theta_planes.refresh()
+            net.add_planes(on)
             inst = self._acting[E] = (buf, on)
         buf, on = inst
         buf.copy_(x.reshape(buf.shape), non_blocking=True)
@@ -383,7 +359,7 @@ class DQNAgent(object):
         """target / online forward passes, TD targets and errors (dqn_agent.py:87-103); kernels and one D2H copy"""
         lib, st = self.lib, _lib.current_stream()
         net = self.networks["main"]
-        if self.head_desc is not None and not self._head_split:
+        if self.head_desc is not None:
             # feature layers of the three bindings, then the fused head launch: Q values, TD targets / errors, head loss,
             # dL/dQ and the head's backward pass (cb200_dqn_head_fused)
             import ctypes
@@ -443,45 +419,20 @@ class DQNAgent(object):
         """the optimizer part of the previous step (own stream) is ordered before whatever the current stream does next"""
         self._side_opt.join()
 
-    def _part_backward(self, weights, with_optimizer, part="all", with_norm=True):
-        """head loss, backward pass, global norm / clipping [, optimizer].  part: "all", or "top" (loss + dense
-        layers) / "bottom" (conv layers + norm) when the all-reduce of the dense gradients overlaps the rest"""
+    def _part_backward(self, weights, with_norm):
+        """head loss, backward pass [, global norm and clipping]"""
         lib, st = self.lib, _lib.current_stream()
         net = self.networks["main"]
-        if self.head_desc is not None and not self._head_split:
+        if self.head_desc is not None:
             # loss, dL/dQ and the head's gradients were produced by the fused head launch of the forward part
             net.online_s.backward_features(side=self._side_w)
-            self._side_w.join()
-            n = net.store.size
-            clip = net.params.clip_gradients
-            if not with_norm:
-                return                                            # the norm is reduced beside the optimizer step
-            if with_optimizer and not (clip is not None and clip != 0) and self._side_w is not NO_SIDE:
-                # no clipping: the gradient norm is only reported -- it is reduced beside the optimizer step
-                self._part_optimizer(1.0, True)
-                return
-            _lib.check(lib.cb200_sumsq(net.store.grad.data_ptr(), n, net.sumsq.data_ptr(), net.ws.ptr(), st))
-            if clip is not None and clip != 0:
-                if net.params.gradients_clipping_method != "ClipByGlobalNorm":
-                    raise NotImplementedError("only ClipByGlobalNorm is implemented on device")
-                _lib.check(lib.cb200_clip_by_global_norm(net.store.grad.data_ptr(), n, net.sumsq.data_ptr(), float(clip),
-                                                         st))
-            if with_optimizer:
-                net.apply_gradients(1.0)
-            return
-        if part != "bottom":
-            self._head_loss_grad(weights, st)
-        if part == "top":
-            net.online_s.backward_top()
-            return
-        if part == "bottom":
-            net.online_s.backward_bottom()
         else:
+            self._head_loss_grad(weights, st)
             net.online_s.backward(side=self._side_w)
-            self._side_w.join()
-        n = net.store.size
+        self._side_w.join()
         if not with_norm:
-            return
+            return                                                # the norm is reduced beside the optimizer step
+        n = net.store.size
         _lib.check(lib.cb200_sumsq(net.store.grad.data_ptr(), n, net.sumsq.data_ptr(), net.ws.ptr(), st))
         clip = net.params.clip_gradients
         if clip is not None and clip != 0:
@@ -489,89 +440,22 @@ class DQNAgent(object):
                 raise NotImplementedError("only ClipByGlobalNorm is implemented on device")
             _lib.check(lib.cb200_clip_by_global_norm(net.store.grad.data_ptr(), n, net.sumsq.data_ptr(), float(clip),
                                                      st))
-        if with_optimizer:
-            net.apply_gradients(1.0)
 
-    def _capture(self, cols, weights, per_libm, single, overlap):
-        c0 = self.lib.cb200_launch_count()
-        ga, gb, gb2 = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph(), None
-        torch.cuda.synchronize()
-        with torch.cuda.graph(ga):
-            self._part_forward(cols, per_libm)
-        c1 = self.lib.cb200_launch_count()
-        if overlap:
-            gb2 = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(gb):
-                self._part_backward(weights, False, "top")
-            with torch.cuda.graph(gb2):
-                self._part_backward(weights, False, "bottom")
-        elif not single and bool(_lib.tune_default("graph_collectives", 0)):
-            # several ranks, NCCL all-reduce captured INSIDE the backward graph: backward -> all-reduce -> rescale + Adam
-            # + plane refresh replay as one graph launch (no eager launches between the graphs of a step)
-            net = self.networks["main"]
-            ws = torch.distributed.get_world_size()
-            scaler = 1.0 / ws if net.params.scale_down_gradients_by_number_of_workers_for_sync_training else 1.0
-            with torch.cuda.graph(gb):
-                self._part_backward(weights, False)
-                torch.distributed.all_reduce(net.store.grad, op=torch.distributed.ReduceOp.SUM)
-                net.apply_gradients(scaler)
-            self._collectives_in_graph = True
-        elif self._side_opt is not NO_SIDE:
-            # backward | optimizer as separate graphs: the optimizer graph is replayed on its own stream (after the
-            # all-reduce when there are several ranks) while the main stream already runs the next sample + gather
-            net = self.networks["main"]
-            clip = net.params.clip_gradients
-            self._norm_in_opt = single and not (clip is not None and clip != 0)
-            scaler = 1.0
-            if not single:
-                ws = torch.distributed.get_world_size()
-                scaler = 1.0 / ws if net.params.scale_down_gradients_by_number_of_workers_for_sync_training else 1.0
-            with torch.cuda.graph(gb):
-                self._part_backward(weights, False, with_norm=not self._norm_in_opt)
-            c2 = self.lib.cb200_launch_count()
-            gc = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(gc):
-                self._part_optimizer(scaler, self._norm_in_opt)
-            c3 = self.lib.cb200_launch_count()
-            self._graph_c = (gc, int(c3 - c2))
-            self._graphs = (ga, gb, gb2, int(c1 - c0), int(c2 - c1))
-            self._opt_on_stream = True
+    def _run(self, k, graph, part, *args):
+        """part k of the learn step: its kernels launched one by one, or (graph) its CUDA graph, recorded the first
+        time and replayed from then on"""
+        if not graph:
+            part(*args)
             return
-        else:
-            with torch.cuda.graph(gb):
-                self._part_backward(weights, single)
-        c2 = self.lib.cb200_launch_count()
-        gc = None
-        if not single and not overlap and not self._collectives_in_graph:
-            # several ranks: the eager NCCL all-reduce sits between the backward graph and a third graph holding the
-            # 1 / world rescale, the Adam step and the refresh of the parameter planes (one launch instead of ~8)
-            net = self.networks["main"]
-            ws = torch.distributed.get_world_size()
-            scaler = 1.0 / ws if net.params.scale_down_gradients_by_number_of_workers_for_sync_training else 1.0
-            gc = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(gc):
-                net.apply_gradients(scaler)
-        c3 = self.lib.cb200_launch_count()
-        self._graph_c = (gc, int(c3 - c2))
-        self._graphs = (ga, gb, gb2, int(c1 - c0), int(c2 - c1))
-
-    def _overlapped_allreduce_begin(self):
-        """dense-layer gradients (the tail of the flat buffer, ~95 % of it) are final: copy them to the exchange
-        buffer and start their all-reduce; it runs on NCCL's stream under the conv backward pass"""
-        net = self.networks["main"]
-        off = net.online_s.grad_split_offset()
-        self._grad_sync[off:].copy_(net.store.grad[off:])
-        return off, torch.distributed.all_reduce(self._grad_sync[off:], async_op=True)
-
-    def _overlapped_allreduce_end(self, off, work):
-        net = self.networks["main"]
-        self._grad_sync[:off].copy_(net.store.grad[:off])
-        work2 = torch.distributed.all_reduce(self._grad_sync[:off], async_op=True)
-        work.wait()
-        work2.wait()
-        ws = torch.distributed.get_world_size()
-        scaler = 1.0 / ws if net.params.scale_down_gradients_by_number_of_workers_for_sync_training else 1.0
-        net.apply_gradients(scaler, grad=self._grad_sync)
+        if len(self._graphs) == k:
+            c0 = self.lib.cb200_launch_count()
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                part(*args)
+            self._graphs.append((g, int(self.lib.cb200_launch_count() - c0)))
+        g, n = self._graphs[k]
+        g.replay()
+        self.graph_kernel_launches += n
 
     def learn_from_batch(self, batch, fetch=True):
         net = self.networks["main"]
@@ -597,80 +481,41 @@ class DQNAgent(object):
             own = own and weights.data_ptr() == self.batch_buffers["weight32"].data_ptr()
         per_libm = per and self.memory.priority_mode == "libm"
         self._head_weights = weights
-        single = not parallel.is_distributed()                    # no all-reduce between backward and optimizer
-        # several ranks, no global-norm clipping (which needs the complete local gradient first), plain Q head: the
-        # all-reduce of the dense layers' gradients can run under the conv backward pass (CB200_DQN_OVERLAP_ALLREDUCE=1).
-        # Bit-identical (tools/check_allreduce_overlap.py); opt-in because the 6.75 MB all-reduce over NVSwitch is short
-        # against the two extra copies and launches it needs.
-        clip = net.params.clip_gradients
-        overlap = (not single) and not (clip is not None and clip != 0) and not self.net_def.dueling and \
-            bool(_lib.tune_default("dqn_overlap_allreduce", 0))
-        self._head_split = overlap          # the overlapped all-reduce needs the head's backward as a separate part
-        if overlap and self._grad_sync is None:
-            self._grad_sync = torch.zeros_like(net.store.grad)
         graph = self.use_graph and own and self._eager_steps >= 2
         self._join_optimizer()             # the previous step's Adam / plane refresh (own stream) comes first
         if graph and self._graphs is None:
-            self._capture(cols, weights, per_libm, single, overlap)
+            self._graphs = []              # this step records the graphs of its parts
+        # one rank and no clipping: the gradient norm is only reported, so a replayed step reduces it beside the
+        # optimizer step, which runs on its own stream (ordered after the all-reduce, joined lazily).  Eager steps are
+        # bound by host time, where those forks and joins cost more than they overlap (CartPole): they keep the norm
+        # and the optimizer on the caller's stream.
+        clip = net.params.clip_gradients
+        norm_in_opt = graph and not parallel.is_distributed() and not (clip is not None and clip != 0)
+        self._run(0, graph, self._part_forward, cols, per_libm)
         ev = None
-        pending = None
-        if graph:
-            ga, gb, gb2, na, nb = self._graphs
-            ga.replay()
-            if per_libm:
-                ev = torch.cuda.Event()
-                ev.record()
-            gb.replay()
-            if gb2 is not None:
-                pending = self._overlapped_allreduce_begin()
-                gb2.replay()
-            self.graph_kernel_launches += na + nb
-        else:
-            self._part_forward(cols, per_libm)
-            if per_libm:
-                ev = torch.cuda.Event()
-                ev.record()
-            if overlap:
-                self._part_backward(weights, False, "top")
-                pending = self._overlapped_allreduce_begin()
-                self._part_backward(weights, False, "bottom")
-            else:
-                self._part_backward(weights, False)
+        if per_libm:
+            ev = torch.cuda.Event()
+            ev.record()
+        self._run(1, graph, self._part_backward, weights, not norm_in_opt)
+        scaler = parallel.allreduce_gradients(net.store.grad,
+                                              net.params.scale_down_gradients_by_number_of_workers_for_sync_training)
+        with self._side_opt if graph else NO_SIDE:
+            self._run(2, graph, self._part_optimizer, scaler, norm_in_opt)
+        if not graph:
             self._eager_steps += 1
-        if pending is not None:
-            self._overlapped_allreduce_end(*pending)
-        elif graph and self._opt_on_stream:
-            if not single:
-                # (the all-reduce stays on the main stream rather than being issued from the optimizer's stream, beside
-                # the next sample + gather)
-                torch.distributed.all_reduce(net.store.grad, op=torch.distributed.ReduceOp.SUM)
-            with self._side_opt:                                  # ordered after the backward graph; joined lazily
-                self._graph_c[0].replay()
-            self.graph_kernel_launches += self._graph_c[1]
-        elif graph and self._collectives_in_graph:
-            pass                                                  # all-reduce and optimizer ran inside the graph
-        elif graph and not single and self._graph_c[0] is not None:
-            torch.distributed.all_reduce(net.store.grad, op=torch.distributed.ReduceOp.SUM)
-            self._graph_c[0].replay()
-            self.graph_kernel_launches += self._graph_c[1]
-        elif not (graph and single):
-            scaler = parallel.allreduce_gradients(
-                net.store.grad, net.params.scale_down_gradients_by_number_of_workers_for_sync_training)
-            net.apply_gradients(scaler)
         if per:
             if ev is not None:
                 ev.synchronize()                                  # GPU is busy with the backward pass meanwhile
                 pa, pr = self.memory.host_priorities(self._td_host.numpy())
                 self._pa_host.numpy()[:] = pa
                 self._pr_host.numpy()[:] = pr
-                side = self._side_upd.after(ev) if self._side_upd is not NO_SIDE else NO_SIDE
-                with side:
+                with self._side_upd.after(ev):
                     self._pa_dev.copy_(self._pa_host, non_blocking=True)
                     self._pr_dev.copy_(self._pr_host, non_blocking=True)
                     self.memory.update_priorities_device(cols["idx"], self._pa_dev, self._pr_dev)
             else:
                 self.memory.update_priorities(cols["idx"], self.td_err)
-        if fetch == "loss" and self.head_desc is not None and not self._head_split and self.device.type == "cuda":
+        if fetch == "loss" and self.head_desc is not None:
             # train(): only the loss goes back to the caller.  With the fused head it is final when the forward part is
             # (its D2H copy sits right behind the head launch), so the host returns while the backward pass, the tree
             # update and the optimizer are still running -- the next step's store() / sample preparation overlaps them.
@@ -699,8 +544,7 @@ class DQNAgent(object):
         for _ in range(self.ap.algorithm.num_consecutive_training_steps):
             self.training_iteration += 1
             batch = self.sample_batch()
-            total_loss, losses, unclipped_grads = self.learn_from_batch(
-                batch, fetch=("loss" if self._early_loss else True) if fetch else False)
+            total_loss, losses, unclipped_grads = self.learn_from_batch(batch, fetch="loss" if fetch else False)
             loss = loss + total_loss if fetch else total_loss
             net = self.networks["main"]
             if net.has_target and self._should_update_online_weights_to_target():

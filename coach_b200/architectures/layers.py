@@ -109,6 +109,14 @@ class _NoSide(object):
 NO_SIDE = _NoSide()
 
 
+def _derive(layer, w):
+    """a prepared layer is ready to run: its weight-derived operands are derived from the weights as they are now
+    (layer.run_perms; after a later write of the weights ThetaPlanes.refresh runs it again).  Host-side tests prepare
+    layers over CPU tensors only to inspect their tables: nothing is launched for them."""
+    if w.is_cuda:
+        layer.run_perms()
+
+
 def _u8_div(lut, x_is_u8):
     return float(getattr(lut, "u8_div", 0.0)) if (x_is_u8 and lut is not None) else 0.0
 
@@ -301,12 +309,14 @@ class Dense(object):
             self.bwd_x = tl.masked_forward_op(lib, ws, B, device, pl.dy, N, self.wT_planes, Ca,
                                               [[(0, q)] for q in range(npix)], npix, dx, Ca,
                                               x if prev_act else None, prev_act, rowmap, pl.dx, mask_planes=pl.x)
+        _derive(self, w)
 
     def forward(self):
         self.fwd.run()
 
     def run_perms(self):
-        """weight-derived operands of this layer: the per-pixel transposed kernels of the data-gradient GEMM"""
+        """weight-derived operands of this layer: the per-pixel transposed kernels of the data-gradient GEMM (run when
+        the layer is prepared and by ThetaPlanes.refresh after every write of the weights)"""
         if self.tiled_x and getattr(self, "perm", None) is not None:
             _lib.check(self.lib.cb200_permute_f32(self.w.data_ptr(), self.perm.data_ptr(), self.perm.numel(),
                                                   self.wT.data_ptr(), self.wT_planes.ptr, self.wT_planes.stride,
@@ -320,14 +330,10 @@ class Dense(object):
                     dy, B, N, db = self.db_args
                     _lib.check(self.lib.cb200_colsum(dy.data_ptr(), B, N, db.data_ptr(), self.ws.side().ptr(),
                                                      _lib.current_stream()))
-        st = _lib.current_stream()
         if self.bwd_x is not None:
-            if self.tiled_x:
-                if not getattr(self, "perms_managed", False):
-                    self.run_perms()
-            else:
+            if not self.tiled_x:          # (the tiled form's transposed kernels are derived by run_perms)
                 _lib.check(self.lib.cb200_transpose(self.w.data_ptr(), self.K, self.N, self.wT.data_ptr(), None, 0,
-                                                    st))
+                                                    _lib.current_stream()))
             self.bwd_x.run()
 
 
@@ -477,6 +483,7 @@ class Conv2d(object):
             if not fused:
                 self.db_args = (dy, B * nq, N, db)
                 ws.require(1024 * N)
+        _derive(self, w)
 
     def _prepare_tiled(self, lib, ws, B, device, x, y, w, b, dw, db, dy, dx, need_dx, prev_act, pl):
         """input available as planes [H * W * B, C]: forward, weight gradient and data gradient as multi-tap GEMMs"""
@@ -523,6 +530,7 @@ class Conv2d(object):
         rowmap_in = _dev_i32((bb * npix + qq).reshape(-1), device)
         self.bwd_x = tl.masked_forward_op(lib, ws, B, device, pl.dy, N, self.wT_planes, C, lists, npix, dx, C,
                                           x if prev_act else None, prev_act, rowmap_in, pl.dx, mask_planes=pl.x)
+        _derive(self, w)
 
     def forward(self):
         if self.s2d is not None:
@@ -530,13 +538,12 @@ class Conv2d(object):
             x, xp, B = self.s2d
             if x is not None:
                 _lib.check(self.lib.cb200_u8_s2d_planes(x.data_ptr(), B, self.H, self.W, self.C, self.S, xp.ptr, st))
-            if not getattr(self, "perms_managed", False):
-                self.run_perms()
         self.fwd.run()
 
     def run_perms(self):
         """weight-derived operands of this layer: the space-to-depth kernel (forward) and the per-tap transposed
-        kernels of the data-gradient GEMM"""
+        kernels of the data-gradient GEMM (run when the layer is prepared and by ThetaPlanes.refresh after every write
+        of the weights)"""
         st = _lib.current_stream()
         if self.s2d is not None:
             _lib.check(self.lib.cb200_permute_f32(self.w.data_ptr(), self.w_perm.data_ptr(), self.w_perm.numel(),
@@ -561,9 +568,4 @@ class Conv2d(object):
                                                   None, 0, 0, st))
             op.run()
         if self.bwd_x is not None:
-            if not getattr(self, "perms_managed", False):
-                st2 = _lib.current_stream()
-                _lib.check(self.lib.cb200_permute_f32(self.w.data_ptr(), self.perm.data_ptr(), self.perm.numel(),
-                                                      self.wT.data_ptr(), self.wT_planes.ptr, self.wT_planes.stride,
-                                                      self.wT_planes.cols, st2))
             self.bwd_x.run()

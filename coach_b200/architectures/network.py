@@ -212,7 +212,7 @@ class SequentialInstance(object):
 
     def backward(self, weights=True, layers=None, side=None):
         """weights=False: data gradients only (d(out)/d(input), e.g. dQ/da through the critic).  layers=(lo, hi): only
-        layers lo <= i < hi, last first (lets a caller start the all-reduce of the top layers' gradients early)."""
+        layers lo <= i < hi, last first (e.g. everything below a head the caller differentiates itself)."""
         lo, hi = (0, len(self.layers)) if layers is None else layers
         for i in reversed(range(lo, hi)):
             if side is not None:

@@ -47,7 +47,6 @@ class QNetworkDef(object):
         else:
             layers.append(Dense(self.obs_shape[0], 256, "relu"))
             flat = 256
-        self.n_embedder = len(layers)
         for u in self.middleware_units:
             layers.append(Dense(flat, u, "relu"))
             flat = u
@@ -75,9 +74,8 @@ class QNetworkInstance(object):
         self.net, self.lib, self.B = net, lib, B
         dev = net.device
         x_is_u8 = isinstance(x, tl.PlaneBuf) or x.dtype == torch.uint8      # PlaneBuf: s2d plane of the uint8 frames
-        # Large batches run the trunk on pre-split bf16 operands (architectures/tiled.py).  The parameter planes are
-        # re-derived from theta at the start of every forward (one launch), so any writer of theta -- Adam, a target
-        # network copy, polyak, a checkpoint load -- is covered.
+        # Large batches run the trunk on pre-split bf16 operands (architectures/tiled.py).  Whoever writes theta --
+        # Adam, a target network copy, polyak, a checkpoint load -- calls theta_planes.refresh() right after the write.
         # (CB200_GEMM_TILED=0 keeps every layer on the gather-GEMM of cb200_gemm: A/B runs, bench.py --no-tc)
         self.theta_planes = tl.ThetaPlanes(lib, net.store, theta) \
             if (B >= 128 and B % 32 == 0 and _lib.tune_default("gemm_tiled", 1)) else None
@@ -88,23 +86,29 @@ class QNetworkInstance(object):
                                      net.is_image and tl.channels_ok(last.N) and tl.width_ok(last.N))
         self.trunk = net.trunk.instantiate(lib, ws, B, x, theta, grad, x_is_u8=x_is_u8, lut=net.lut, train=train,
                                            theta_planes=self.theta_planes, last_planes=self.towers_on_planes)
+        self.towers_dx = None
         if not net.dueling:
             self.q = self.trunk.out
             self.dq = self.trunk.d_out
-            return
-        h = self.trunk.out                      # what the head reads (post-ReLU): middleware or embedder output
-        dh = self.trunk.d_out                   # gradient wrt its pre-activation
-        relu = 1
-        self.q = torch.empty((B, net.num_actions), dtype=torch.float32, device=dev)
-        self.dq = torch.empty_like(self.q) if train else None
-        self.towers_dx = None
-        if self.towers_on_planes:
-            self._towers_on_conv_map(lib, ws, B, h, dh, theta, grad, train)
-            return
-        self.v = net.v_tower.instantiate(lib, ws, B, h, theta, grad, need_input_grad=train, input_act=relu,
-                                         train=train, dx_in=dh, dx_accumulate=False)
-        self.a = net.a_tower.instantiate(lib, ws, B, h, theta, grad, need_input_grad=train, input_act=relu,
-                                         train=train, dx_in=dh, dx_accumulate=True)
+        else:
+            h = self.trunk.out                  # what the head reads (post-ReLU): middleware or embedder output
+            dh = self.trunk.d_out               # gradient wrt its pre-activation
+            self.q = torch.empty((B, net.num_actions), dtype=torch.float32, device=dev)
+            self.dq = torch.empty_like(self.q) if train else None
+            if self.towers_on_planes:
+                self._towers_on_conv_map(lib, ws, B, h, dh, theta, grad, train)
+            else:
+                self.v = net.v_tower.instantiate(lib, ws, B, h, theta, grad, need_input_grad=train, input_act=1,
+                                                 train=train, dx_in=dh, dx_accumulate=False)
+                self.a = net.a_tower.instantiate(lib, ws, B, h, theta, grad, need_input_grad=train, input_act=1,
+                                                 train=train, dx_in=dh, dx_accumulate=True)
+        if self.theta_planes is not None:
+            # kernels derived from the weights (per-tap transposed kernels of the data-gradient GEMMs, the
+            # space-to-depth kernel of the first convolution) are re-derived together with the planes
+            for sq in [self.trunk] + ([self.v, self.a] if net.dueling else []):
+                self.theta_planes.derived += [layer.run_perms for layer in sq.layers]
+            if self.towers_dx is not None:
+                self.theta_planes.derived.append(self._towers_perm)
 
     def _towers_on_conv_map(self, lib, ws, B, h, dh, theta, grad, train):
         """V / A towers as tiled GEMMs on the planes of the last conv map [npix * B, C].  Forward and weight gradients
@@ -148,14 +152,7 @@ class QNetworkInstance(object):
             _lib.check(self.lib.cb200_permute_f32(w.data_ptr(), perm.data_ptr(), perm.numel(),
                                                   wT.data_ptr() + 4 * t * perm.numel(), pv.ptr, pv.stride, pv.cols, st))
 
-    def _run_towers_dx(self):
-        if not getattr(self, "_towers_perm_managed", False):
-            self._towers_perm()
-        self.towers_dx[0].run()
-
     def forward(self):
-        if self.theta_planes is not None:
-            self.theta_planes.refresh_if_auto()
         self.trunk.forward()
         if self.net.dueling:
             self.v.forward()
@@ -176,8 +173,6 @@ class QNetworkInstance(object):
 
     def forward_features(self):
         """everything below the head: the feature layer's post-ReLU output is ``features``"""
-        if self.theta_planes is not None:
-            self.theta_planes.refresh_if_auto()
         self.trunk.forward(upto=len(self.trunk.layers) - 1)
         return self.trunk.acts[-2]
 
@@ -185,37 +180,6 @@ class QNetworkInstance(object):
         """expects the gradient w.r.t. the feature layer's pre-activation in trunk.dzs[-2] (/ its planes).
         side: a layers.SideStream for the weight-gradient launches (they leave the data-gradient chain)"""
         self.trunk.backward(layers=(0, len(self.trunk.layers) - 1), side=side)
-
-    def manage_planes(self):
-        """the owner takes over refreshing the parameter planes: the layers' weight permutes (per-tap transposed
-        kernels, space-to-depth kernel) move from every forward / backward pass into ThetaPlanes.refresh()"""
-        if self.theta_planes is None:
-            return False
-        self.theta_planes.auto = False
-        seqs = [self.trunk] + ([self.v, self.a] if self.net.dueling else [])
-        for sq in seqs:
-            for layer in sq.layers:
-                if hasattr(layer, "run_perms") and not getattr(layer, "perms_managed", False):
-                    layer.perms_managed = True
-                    self.theta_planes.derived.append(layer.run_perms)
-        if getattr(self, "towers_dx", None) is not None and not getattr(self, "_towers_perm_managed", False):
-            self._towers_perm_managed = True
-            self.theta_planes.derived.append(self._towers_perm)
-        return True
-
-    def backward_top(self):
-        """plain Q head only: the dense layers (middleware + head) of the trunk, which hold ~95 % of the parameters;
-        their gradients are complete -- and can be all-reduced -- while ``backward_bottom`` still runs"""
-        assert not self.net.dueling
-        n = len(self.trunk.layers)
-        self.trunk.backward(layers=(self.net.n_embedder, n))
-
-    def backward_bottom(self):
-        self.trunk.backward(layers=(0, self.net.n_embedder))
-
-    def grad_split_offset(self):
-        """element offset in the flat gradient buffer where the top (dense) layers' gradients start"""
-        return self.net.store.entries[self.net.trunk.names[self.net.n_embedder][0]][0]
 
     def backward(self, side=None):
         """expects d(loss)/dq in self.dq; leaves all parameter gradients in the grad buffer"""
@@ -226,5 +190,5 @@ class QNetworkInstance(object):
             self.v.backward(side=side)      # writes d(middleware pre-activation)
             self.a.backward(side=side)      # accumulates into it
             if self.towers_dx is not None:
-                self._run_towers_dx()      # both towers' data gradients into the conv map, one GEMM
+                self.towers_dx[0].run()     # both towers' data gradients into the conv map, one GEMM
         self.trunk.backward(side=side)

@@ -3,7 +3,7 @@
 The tensor-core path of the learn step computes fp32 products as 3 x BF16 operand splits.  Splitting inside every GEMM
 costs more than the GEMM, so every tensor that feeds a GEMM is kept, next to its fp32 form, as three bf16 "planes" in
 the 8x8 core-tiled format of csrc/nn_gemm.cuh (``tiled_elem``): activations / gradients as [pixel * batch + b, channel]
-matrices written by the producing GEMM's epilogue, parameters re-derived from theta once per forward
+matrices written by the producing GEMM's epilogue, parameters re-derived from theta after every write of it
 (``ThetaPlanes.refresh``), per-tap transposed kernels by the permute kernel.  ``build_*`` below turn a layer geometry
 into the tap lists of cb200_gemm_tiled:
 
@@ -114,16 +114,13 @@ def width_ok(n):
 
 class ThetaPlanes(object):
     """Planes of every 2-D-able kernel of a flat parameter buffer, at the kernels' own element offsets.  ``refresh``
-    re-derives all of them from the current fp32 values in one launch (start of every forward: covers Adam, target
-    network copies, polyak, checkpoint loads)."""
+    re-derives all of them from the current fp32 values in one launch; whoever writes theta (Adam, target network
+    copies, polyak, checkpoint loads) calls it right after the write."""
 
     def __init__(self, lib, store, theta):
         self.lib, self.store, self.theta = lib, store, theta
-        # auto: every forward pass re-derives the planes (safe for any writer of theta).  An owner that knows every
-        # writer -- the DQN agent: Adam, target copies -- switches it off and calls refresh() right after each write;
-        # `derived` are further kernels over theta (transposed / permuted kernels of the data-gradient GEMMs, the
-        # space-to-depth kernel of the first convolution) that then run with the refresh instead of in every pass.
-        self.auto = True
+        # further kernels over theta that run with the refresh: transposed / permuted kernels of the data-gradient
+        # GEMMs, the space-to-depth kernel of the first convolution
         self.derived = []
         # one buffer of 6 * size elements.  Planar kernels: plane p of the tensor at `off` sits at p * size + off
         # (first half).  Row-group interleaved kernels (narrow B operands, ``b_interleaved``): [3 off, 3 off + 3 rows
@@ -166,31 +163,13 @@ class ThetaPlanes(object):
     def stride(self):
         return self.store.size
 
-    def refresh_if_auto(self):
-        if self.auto:
-            self.refresh()
-
     def refresh(self):
-        if len(self.derived) > 1 and self.theta.is_cuda and _lib.tune_default("refresh_streams", 0):
-            # the derived kernels (weight permutes) and the plane split are independent readers of theta: two side
-            # streams next to the caller's (parallel branches when the caller is being captured into a CUDA graph).
-            # Opt-in: the fork / join can cost more than the five small kernels gain from running side by side.
-            from coach_b200.architectures.layers import SideStream
-            if getattr(self, "_sides", None) is None:
-                self._sides = (SideStream(self.theta.device), SideStream(self.theta.device))
-            for k, side in enumerate(self._sides):
-                with side:
-                    for fn in self.derived[k::2]:
-                        fn()
-        else:
-            for fn in self.derived:
-                fn()
+        for fn in self.derived:
+            fn()
         if self.segs is not None:
             _lib.check(self.lib.cb200_split_planes(self.theta.data_ptr(), self.planes.data_ptr(), self.stride,
                                                    self.segs.data_ptr(), self.segs.shape[0], self.max_elems,
                                                    _lib.current_stream()))
-        for side in (getattr(self, "_sides", None) or ()):
-            side.join()
 
 
 class PlaneCtx(object):

@@ -167,7 +167,7 @@ def restore_memory(mem, prefix):
 
 
 def _network_items(agent):
-    """(tag, ParamStore, extra tensors {name: tensor}, host state {name: value}) for every network of an agent"""
+    """(tag, ParamStore, extra tensors {name: tensor}, owner) for every network of an agent"""
     out = []
     nets = getattr(agent, "networks", None)
     if isinstance(nets, dict) and "main" in nets and hasattr(nets["main"], "store"):          # DQN family
@@ -175,13 +175,13 @@ def _network_items(agent):
         extra = {"adam_state": w.adam_state}
         if w.theta_target is not None:
             extra["target"] = w.theta_target
-        out.append(("main", w.store, extra, {"beta1_power": float(w.beta1_power), "beta2_power": float(w.beta2_power)}, w))
+        out.append(("main", w.store, extra, w))
     for tag in ("actor", "critic", "policy", "q", "v"):                                       # _Net based agents
         net = getattr(agent, tag, None)
         if net is not None and hasattr(net, "store") and hasattr(net, "adam_state"):
-            out.append((tag, net.store, {"adam_state": net.adam_state, "target": net.target}, {}, net))
+            out.append((tag, net.store, {"adam_state": net.adam_state, "target": net.target}, net))
     if hasattr(agent, "net") and hasattr(agent.net, "store") and hasattr(agent, "theta_target"):   # ClippedPPO
-        out.append(("main", agent.net.store, {"adam_state": agent.adam_state, "target": agent.theta_target}, {}, agent))
+        out.append(("main", agent.net.store, {"adam_state": agent.adam_state, "target": agent.theta_target}, agent))
     return out
 
 
@@ -199,7 +199,7 @@ def save_checkpoint(agent, checkpoint_dir: str, checkpoint_id: int = 0, env_step
                                                         ("training_iteration", "total_steps_counter",
                                                          "last_target_network_update_step", "last_training_phase_step")
                                                         if hasattr(agent, k)}, "networks": {}}
-    for tag, store, extra, host, _ in _network_items(agent):
+    for tag, store, extra, _ in _network_items(agent):
         base = "%s.net_%s" % (prefix, tag)
         for nm, t in (("theta", store.theta), ("m", store.m), ("v", store.v)):
             _save_tensor("%s.%s.npy" % (base, nm), t)
@@ -207,7 +207,7 @@ def save_checkpoint(agent, checkpoint_dir: str, checkpoint_id: int = 0, env_step
             _save_tensor("%s.%s.npy" % (base, nm), t)
         meta["networks"][tag] = {"size": int(store.size), "entries": [[n, int(o), list(s)] for n, (o, s) in
                                                                       store.entries.items()],
-                                 "extra": sorted(extra), "host": host}
+                                 "extra": sorted(extra)}
     if getattr(agent, "memory", None) is not None and hasattr(agent.memory, "ring"):
         save_memory(agent.memory, prefix)
     flt = getattr(agent, "pre_network_filter", None)
@@ -232,7 +232,7 @@ def restore_checkpoint(agent, checkpoint_dir: str, name: str = None) -> str:
         meta = json.load(f)
     if meta["agent"] != type(agent).__name__:
         raise ValueError("checkpoint was written by a %s, this is a %s" % (meta["agent"], type(agent).__name__))
-    for tag, store, extra, host, owner in _network_items(agent):
+    for tag, store, extra, owner in _network_items(agent):
         m = meta["networks"][tag]
         if m["size"] != store.size or [e[0] for e in m["entries"]] != list(store.entries):
             raise ValueError("network %r: parameter layout differs from the checkpoint's" % tag)
@@ -241,8 +241,13 @@ def restore_checkpoint(agent, checkpoint_dir: str, name: str = None) -> str:
             _load_into("%s.%s.npy" % (base, nm), t)
         for nm, t in extra.items():
             _load_into("%s.%s.npy" % (base, nm), t)
-        for k, v in m["host"].items():
-            setattr(owner, k, np.float32(v))
+        host = m.get("host")
+        if host:
+            # a DQN checkpoint written while eager agents kept their Adam powers on the host ({beta1 power, beta2
+            # power}): only one of the two copies ever advanced (host: eager agent, device: CUDA-graph agent), and both
+            # only decrease from the betas
+            old = torch.tensor(list(host.values()), dtype=torch.float32)
+            extra["adam_state"].copy_(torch.minimum(extra["adam_state"].cpu(), old))
         # operand planes / derived kernels follow the parameters
         for hook in ("online_changed", "target_changed"):
             if hasattr(owner, hook):

@@ -45,24 +45,58 @@ def _steps(agent, k, seed):
     return out
 
 
+def _as_legacy_format(agent, path, name):
+    """rewrites a DQN checkpoint the way it was written while eager agents kept their Adam powers on the host: the
+    advanced powers in the metadata, the device copy (adam_state.npy) at its initial betas.  Returns the powers."""
+    import json
+    prefix = os.path.join(path, name)
+    state = prefix + ".net_main.adam_state.npy"
+    powers = np.load(state)
+    p = agent.networks["main"].params
+    np.save(state, np.array([p.adam_optimizer_beta1, p.adam_optimizer_beta2], dtype=np.float32))
+    with open(prefix + ".agent.json") as f:
+        meta = json.load(f)
+    meta["networks"]["main"]["host"] = {"beta1_power": float(powers[0]), "beta2_power": float(powers[1])}
+    with open(prefix + ".agent.json", "w") as f:
+        json.dump(meta, f)
+    return powers
+
+
 def test_dqn_agent_continues_bit_identically_after_restore(tmp_path):
+    _check_continuation(tmp_path, B=128, legacy=False)
+
+
+@pytest.mark.parametrize("legacy", [False, True], ids=["current_format", "legacy_format"])
+def test_eager_dqn_agent_continues_bit_identically_after_restore(tmp_path, legacy):
+    """B = 32: every step eager (Adam's step state on the device as in the CUDA-graph steps)"""
+    _check_continuation(tmp_path, B=32, legacy=legacy)
+
+
+def _check_continuation(tmp_path, B, legacy):
     from coach_b200 import checkpoint
-    a = _dqn()
+    a = _dqn(B=B)
     _fill(a, 700, 1)                                   # ring not full: only the live rows are written
-    _steps(a, 4, 50)                                   # eager steps + CUDA-graph capture + a replay
+    _steps(a, 4, 50)                                   # B = 128: eager steps + CUDA-graph capture + a replay
+    assert (a._graphs is not None) == (B >= 128)
     a.total_steps_counter = 1234
     name = checkpoint.save_checkpoint(a, str(tmp_path), checkpoint_id=3)
     assert name == "3_Step-1234.ckpt" and checkpoint.read_state_file(str(tmp_path)) == name
+    adam_state = a.networks["main"].adam_state.clone()
+    if legacy:
+        powers = _as_legacy_format(a, str(tmp_path), name)
+        assert np.array_equal(powers, adam_state.cpu().numpy()) and powers[0] < np.float32(0.9)
     want = _steps(a, 3, 80)
     theta_want = a.net_def.store.theta.clone()
     tree_want = a.memory.sum_tree.clone()
-    b = _dqn(seed=99)                                  # different initial weights, empty replay
+    b = _dqn(seed=99, B=B)                             # different initial weights, empty replay
     checkpoint.restore_checkpoint(b, str(tmp_path))
     assert b.total_steps_counter == 1234 and b.memory.num_transitions() == a.memory.num_transitions()
+    assert torch.equal(b.networks["main"].adam_state, adam_state)
     got = _steps(b, 3, 80)
     for (lw, iw), (lg, ig) in zip(want, got):
         assert lw == lg and torch.equal(iw, ig)
     assert torch.equal(b.net_def.store.theta, theta_want) and torch.equal(b.memory.sum_tree, tree_want)
+    assert torch.equal(b.networks["main"].adam_state, a.networks["main"].adam_state)
     assert float(b.memory.beta.current_value) == float(a.memory.beta.current_value)
     with pytest.raises(FileNotFoundError):
         checkpoint.restore_checkpoint(b, str(tmp_path / "nothing_here"))
