@@ -63,6 +63,22 @@ class DqnHeadDesc(ctypes.Structure):
                 ("dh_plane_stride", c_i64), ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p)]
 
 
+class EnsembleHeadDesc(ctypes.Structure):
+    """struct cb200_ensemble_head_desc"""
+    _fields_ = [("h_next", c_void_p), ("h_online", c_void_p), ("h_select", c_void_p), ("w_target", c_void_p),
+                ("b_target", c_void_p), ("w_online", c_void_p), ("b_online", c_void_p), ("actions", c_void_p),
+                ("rewards", c_void_p), ("game_overs", c_void_p), ("masks", c_void_p), ("discount", c_double),
+                ("huber", ctypes.c_int32), ("batch", c_i64), ("features", ctypes.c_int32), ("heads", ctypes.c_int32),
+                ("n_actions", ctypes.c_int32), ("grad_rescale", c_float), ("q_online", c_void_p),
+                ("q_next", c_void_p), ("q_select", c_void_p), ("targets", c_void_p), ("dq", c_void_p),
+                ("losses", c_void_p), ("loss", c_void_p), ("dh", c_void_p), ("dh_planes", c_void_p),
+                ("dh_plane_stride", c_i64), ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p)]
+
+
+# cb200_ensemble_action_values modes
+ENSEMBLE_SELECT, ENSEMBLE_UCB, ENSEMBLE_MEAN, ENSEMBLE_VOTE = 0, 1, 2, 3
+
+
 class Column(ctypes.Structure):
     """struct cb200_column"""
     _fields_ = [("src", c_void_p), ("dst", c_void_p), ("row_bytes", c_i64)]
@@ -112,6 +128,9 @@ PROTOTYPES = {
     "cb200_regression_head_loss_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_i64, c_int, c_float, c_void_p,
                                                 c_void_p, c_void_p]),
     "cb200_dqn_head_fused": (c_int, [c_void_p, c_void_p]),
+    "cb200_ensemble_head_fused": (c_int, [c_void_p, c_void_p]),
+    "cb200_ensemble_action_values": (c_int, [c_void_p, c_i64, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, c_void_p,
+                                             c_float, c_void_p, c_void_p]),
     "cb200_dueling_combine_fwd": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p, c_void_p]),
     "cb200_dueling_combine_bwd": (c_int, [c_void_p, c_i64, c_i64, c_void_p, c_void_p, c_void_p]),
     "cb200_sumsq": (c_int, [c_void_p, c_i64, c_void_p, c_void_p, c_void_p]),

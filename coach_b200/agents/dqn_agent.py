@@ -178,19 +178,24 @@ class DQNAgent(object):
             "weight": torch.ones(B, dtype=torch.float64, device=dev),
             "weight32": torch.ones(B, dtype=torch.float32, device=dev),
         }
+        extra = self._extra_columns()
+        self.batch_buffers.update(extra)
+        # columns whose persistent buffers a batch must use for the CUDA-graph replay (fixed pointers in the graphs)
+        self._own_columns = ("action", "reward", "game_over") + tuple(extra)
         # the ring's column layout = the agent's batch buffers, fixed before the first store: store(Transition) then
         # casts what the environment hands out (gym: float64) instead of the gather overrunning float32 buffers
         if hasattr(self.memory, "declare_schema") and self.memory.ring.specs is None:
             img = ("state:observation", "next_state:observation") if len(self.observation_shape) == 3 else ()
             self.memory.declare_schema({k: self.batch_buffers[k] for k in
                                         ("state:observation", "next_state:observation", "action", "reward",
-                                         "game_over")}, image_columns=img)
+                                         "game_over") + tuple(extra)}, image_columns=img)
         dueling = "DuelingQHead" in getattr(net_params, "heads_parameters", ["QHead"])
         gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
         scheme = getattr(getattr(net_params, "middleware_parameters", None), "scheme", MiddlewareScheme.Medium)
         self.head_outputs = self._head_outputs()      # width of the head's output layer (C51: actions x atoms)
         self.net_def = QNetworkDef(dev, self.observation_shape, self.head_outputs, dueling=dueling,
-                                   middleware_units=MiddlewareScheme.units[getattr(scheme, "value", scheme)])
+                                   middleware_units=MiddlewareScheme.units[getattr(scheme, "value", scheme)],
+                                   **self._head_kwargs())
         self.net_def.store.init_glorot(gen)
         # Fused input path (image observations on the tensor-core path): the replay's sample kernel writes the
         # space-to-depth bf16 plane the first convolution contracts -- no staged uint8 copy, no conversion pass.
@@ -212,9 +217,7 @@ class DQNAgent(object):
         # plain Q head: head forward passes, TD targets, loss and the head's backward pass are ONE fused launch
         net = self.networks["main"]
         self.head_desc = None
-        if (_lib.tune_default("fused_head", 1) and dev.type == "cuda" and net.has_target and
-                net.online_s.head_fusable() and net.target_s2.head_fusable() and
-                (net.online_s2 is None or net.online_s2.head_fusable())):
+        if _lib.tune_default("fused_head", 1) and dev.type == "cuda" and net.has_target and self._head_fusable(net):
             self._build_head_desc()
         self.targets = torch.zeros((B, self.head_outputs), dtype=torch.float32, device=dev)
         self.td_err = torch.zeros(B, dtype=torch.float64, device=dev)
@@ -257,6 +260,19 @@ class DQNAgent(object):
 
     def _head_outputs(self):
         return self.num_actions
+
+    def _head_kwargs(self):
+        """extra QNetworkDef arguments of the head (Bootstrapped DQN: head copies)"""
+        return {}
+
+    def _extra_columns(self):
+        """replay columns beyond the transition's five, as {name: persistent batch buffer} (Bootstrapped DQN: the
+        bootstrap masks); they join the ring's schema and the own-buffer check of the CUDA-graph replay"""
+        return {}
+
+    def _head_fusable(self, net):
+        return (net.online_s.head_fusable() and net.target_s2.head_fusable() and
+                (net.online_s2 is None or net.online_s2.head_fusable()))
 
     # ---- reference plumbing ------------------------------------------------------------------------------------------
     @property
@@ -461,7 +477,7 @@ class DQNAgent(object):
         net = self.networks["main"]
         cols = batch.columns
         img = ("state:observation", "next_state:observation")
-        own = all(cols[k].data_ptr() == self.batch_buffers[k].data_ptr() for k in ("action", "reward", "game_over"))
+        own = all(cols[k].data_ptr() == self.batch_buffers[k].data_ptr() for k in self._own_columns)
         for k in img:
             if self.s2d is not None:
                 if k in cols:      # a batch that carries uint8 frames (not sampled through the fused path): convert

@@ -25,6 +25,8 @@ class ParamStore(object):
         self.entries = OrderedDict()      # name -> (offset, shape)
         self.size = 0
         self.theta = None
+        self.glorot_fans = {}             # kernel name -> (fan_in, fan_out) when it is not the tensor's own
+        self.initial_values = {}          # rescaler name -> initial value (default 1.0)
 
     def add(self, name, shape):
         if self.theta is not None:
@@ -64,11 +66,12 @@ class ParamStore(object):
                     fan_in, fan_out = rf * shape[2], rf * shape[3]
                 else:
                     fan_in, fan_out = shape[0], shape[1]
+                fan_in, fan_out = self.glorot_fans.get(name, (fan_in, fan_out))
                 limit = float(np.sqrt(6.0 / (fan_in + fan_out)))
                 cpu = (torch.rand(shape, generator=generator, dtype=torch.float32) * 2 - 1) * limit
                 v.copy_(cpu)
             elif name.endswith("rescalers"):
-                v.fill_(1.0)
+                v.fill_(self.initial_values.get(name, 1.0))
             else:
                 v.zero_()
 

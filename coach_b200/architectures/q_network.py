@@ -23,8 +23,18 @@ from coach_b200.architectures.network import ParamStore, Sequential, make_u8_lut
 class QNetworkDef(object):
     """Parameter layout + layer chain; instances bind it to buffers (see QNetworkInstance)."""
 
-    def __init__(self, device, observation_shape, num_actions, dueling=False, embedder="auto", middleware_units=512):
-        """middleware_units: width of one FC middleware layer, a tuple of widths, or None / () for MiddlewareScheme.Empty"""
+    def __init__(self, device, observation_shape, num_actions, dueling=False, embedder="auto", middleware_units=512,
+                 head_copies=1, head_grad_rescale=1.0):
+        """middleware_units: width of one FC middleware layer, a tuple of widths, or None / () for MiddlewareScheme.Empty.
+        head_copies > 1 (Bootstrapped DQN, bootstrapped_dqn_agent.py:26-30): ``head_copies`` QHeads of ``num_actions``
+        outputs on the same features, as ONE Dense(head_copies * num_actions) whose column block [k A, (k + 1) A) is
+        head k; each block is Glorot-initialised with the fans of its own [F, A] layer, and there is one
+        ``gradients_from_head_0-<k>_rescalers`` scalar per copy, initialised to ``head_grad_rescale``
+        (general_network.py:304-325)."""
+        self.head_copies = int(head_copies)
+        self.head_grad_rescale = float(head_grad_rescale)
+        if self.head_copies > 1 and dueling:
+            raise NotImplementedError("head copies are implemented for the plain QHead only")
         if middleware_units is None:
             middleware_units = ()
         elif isinstance(middleware_units, int):
@@ -52,16 +62,23 @@ class QNetworkDef(object):
             flat = u
         middleware_units = flat                 # width of what the head reads
         if not self.dueling:
-            layers.append(Dense(middleware_units, self.num_actions, None))
+            layers.append(Dense(middleware_units, self.head_copies * self.num_actions, None))
             self.trunk = Sequential(layers, self.store, "main/online/network_0")
             self.v_tower = self.a_tower = None
+            if self.head_copies > 1:
+                self.store.glorot_fans[self.trunk.names[-1][0]] = (middleware_units, self.num_actions)
         else:
             self.trunk = Sequential(layers, self.store, "main/online/network_0")
             self.v_tower = Sequential([Dense(middleware_units, 512, "relu"), Dense(512, 1, None)], self.store,
                                       "main/online/network_0/dueling_q_values_head_0/state_value")
             self.a_tower = Sequential([Dense(middleware_units, 512, "relu"), Dense(512, self.num_actions, None)],
                                       self.store, "main/online/network_0/dueling_q_values_head_0/action_advantage")
-        self.store.add("main/online/network_0/gradients_from_head_0-0_rescalers", ())
+        if self.head_copies == 1:
+            self.store.add("main/online/network_0/gradients_from_head_0-0_rescalers", ())
+        else:
+            for k in range(self.head_copies):
+                name = self.store.add("main/online/network_0/gradients_from_head_0-%d_rescalers" % k, ())
+                self.store.initial_values[name] = self.head_grad_rescale
         self.store.finalize()
         self.lut = make_u8_lut(self.device) if self.is_image else None
 
@@ -170,6 +187,16 @@ class QNetworkInstance(object):
         head = self.trunk.layers[-1]
         return (type(head).__name__ == "Dense" and head.K in (256, 512) and head.N <= 8 and
                 self.trunk.acts[-2] is not None and self.trunk.layers[-2].act == 1)
+
+    def ensemble_fusable(self):
+        """head copies of <= 8 actions each on a 256- or 512-wide feature layer whose fp32 activations are kept
+        (cb200_ensemble_head_fused)"""
+        if self.net.dueling or len(self.trunk.layers) < 2:
+            return False
+        head = self.trunk.layers[-1]
+        return (type(head).__name__ == "Dense" and head.K in (256, 512) and self.net.num_actions <= 8 and
+                head.N == self.net.head_copies * self.net.num_actions and self.trunk.acts[-2] is not None and
+                self.trunk.layers[-2].act == 1)
 
     def forward_features(self):
         """everything below the head: the feature layer's post-ReLU output is ``features``"""

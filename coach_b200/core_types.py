@@ -244,6 +244,9 @@ class DeviceBatch(object):
                 info["idx"] = int(host["idx"][i])
             if "weight" in host:
                 info["weight"] = host["weight"][i]
+            for k in host:
+                if k.startswith("info:"):
+                    info[k[len("info:"):]] = host[k][i]
             out.append(Transition(state=state, action=action, reward=float(host["reward"][i]), next_state=nstate,
                                   game_over=bool(host["game_over"][i]), info=info))
         return out

@@ -165,6 +165,83 @@ __device__ __forceinline__ void head_dot(const float* __restrict__ hrow, const f
     }
 }
 
+// Per-row arithmetic shared by the DQN head and the ensemble head: every lane of the warp evaluates it on identical
+// values (head_dot leaves the same bits in every lane).
+// DDQN / DQN target action (ddqn_agent.py:42-43 / dqn_agent.py:78-79; np.argmax: first maximum) -> target Q of it
+__device__ __forceinline__ float head_q_best(const float (&qs)[kHeadMaxA], const float (&qn)[kHeadMaxA], bool use_sel,
+                                             int A) {
+    float bv = use_sel ? qs[0] : qn[0];
+    float q_best = qn[0];
+#pragma unroll
+    for (int a = 1; a < kHeadMaxA; ++a) {
+        const float sv = use_sel ? qs[a] : qn[a];
+        if (a < A && sv > bv) {
+            bv = sv;
+            q_best = qn[a];
+        }
+    }
+    return q_best;
+}
+// new_target = r + (1.0 - done) * discount * q'[a*]   (dqn_agent.py:100-101; left-to-right, fp64)
+__device__ __forceinline__ double head_td_target(double reward, uint8_t game_over, double discount, float q_best) {
+    const double not_done = __dsub_rn(1.0, game_over ? 1.0 : 0.0);
+    return __dadd_rn(reward, __dmul_rn(__dmul_rn(not_done, discount), (double)q_best));
+}
+// head loss of one row and dL/dQ (head.py:165-177; tf.losses.huber_loss delta = 1 / mean_squared_error)
+__device__ __forceinline__ float head_loss_grad(const float (&qo)[kHeadMaxA], const float (&tgt)[kHeadMaxA], int A,
+                                                int huber, float w, float inv_b, float (&dq)[kHeadMaxA]) {
+    float row = 0.f;
+#pragma unroll
+    for (int a = 0; a < kHeadMaxA; ++a) {
+        dq[a] = 0.f;
+        if (a < A) {
+            const float e = qo[a] - tgt[a];
+            float l, g;
+            if (huber) {
+                const float ae = fabsf(e);
+                const float qq = fminf(ae, 1.0f);
+                l = 0.5f * qq * qq + (ae - qq);
+                g = (ae <= 1.0f) ? e : (e > 0.f ? 1.0f : -1.0f);
+            } else {
+                l = e * e;
+                g = 2.0f * e;
+            }
+            row += l;
+            dq[a] = w * inv_b * g;
+        }
+    }
+    return row;
+}
+// one row of dL/dz, staged lane-strided in the warp's row buffer: lane l takes the KPL consecutive features
+// [l KPL, (l + 1) KPL) and writes them as float4s and / or as whole 16-byte core rows of the three operand planes
+template <int KPL>
+__device__ __forceinline__ void head_store_dz(const float* rowbuf, int lane, int r, int K, float* dh,
+                                              uint16_t* dh_planes, int64_t dh_plane_stride) {
+    float dz[KPL];
+#pragma unroll
+    for (int j = 0; j < KPL / 4; ++j) {
+        const float4 v = *reinterpret_cast<const float4*>(rowbuf + lane * KPL + 4 * j);
+        dz[4 * j] = v.x; dz[4 * j + 1] = v.y; dz[4 * j + 2] = v.z; dz[4 * j + 3] = v.w;
+    }
+    if (dh) {
+        float4* o = reinterpret_cast<float4*>(dh + (size_t)r * K + lane * KPL);
+#pragma unroll
+        for (int j = 0; j < KPL / 4; ++j) o[j] = make_float4(dz[4 * j], dz[4 * j + 1], dz[4 * j + 2], dz[4 * j + 3]);
+    }
+    if (dh_planes) {
+#pragma unroll
+        for (int c8 = 0; c8 < KPL / 8; ++c8) {
+            const float x8[8] = {dz[8 * c8], dz[8 * c8 + 1], dz[8 * c8 + 2], dz[8 * c8 + 3],
+                                 dz[8 * c8 + 4], dz[8 * c8 + 5], dz[8 * c8 + 6], dz[8 * c8 + 7]};
+            const HeadSplit8 sp = head_split8(x8);
+            uint16_t* d = dh_planes + head_tiled_elem((size_t)r, lane * KPL + 8 * c8, K);
+            *reinterpret_cast<uint4*>(d) = sp.h;
+            *reinterpret_cast<uint4*>(d + dh_plane_stride) = sp.m;
+            *reinterpret_cast<uint4*>(d + 2 * dh_plane_stride) = sp.l;
+        }
+    }
+}
+
 template <int KPL>
 __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadParams p) {
     extern __shared__ __align__(16) float head_smem[];     // Wt_online [A][K] | Wt_target [A][K] | row buffers [warps][K]
@@ -198,22 +275,9 @@ __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadPar
         if (use_sel) head_dot<KPL>(p.h_select + (size_t)r * K, wt_on, p.b_online, A, K, lane, hv, qs);
         head_dot<KPL>(p.h_online + (size_t)r * K, wt_on, p.b_online, A, K, lane, hv, qo);    // hv = h_online slice
         // ---- TD target (every lane, identical values) -- dqn_agent.py:92-103 ------------------------------------------
-        int best = 0;
-        float bv = use_sel ? qs[0] : qn[0];                               // ddqn_agent.py:42-43 / dqn_agent.py:78-79
-        float q_best = qn[0];
-#pragma unroll
-        for (int a = 1; a < kHeadMaxA; ++a) {
-            const float sv = use_sel ? qs[a] : qn[a];
-            if (a < A && sv > bv) {                                       // np.argmax: first maximum
-                bv = sv;
-                best = a;
-                q_best = qn[a];
-            }
-        }
-        (void)best;
+        const float q_best = head_q_best(qs, qn, use_sel, A);
         const int64_t act = p.actions[r];
-        const double not_done = __dsub_rn(1.0, p.game_overs[r] ? 1.0 : 0.0);
-        const double y = __dadd_rn(p.rewards[r], __dmul_rn(__dmul_rn(not_done, p.discount), (double)q_best));
+        const double y = head_td_target(p.rewards[r], p.game_overs[r], p.discount, q_best);
         float tgt[kHeadMaxA], dq[kHeadMaxA];
         double td = 0.0;
 #pragma unroll
@@ -224,28 +288,9 @@ __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadPar
                 tgt[a] = (float)y;
             }
         }
-        // ---- head loss and dL/dQ (head.py:165-177; tf.losses.huber_loss delta = 1 / mean_squared_error) ---------------
+        // ---- head loss and dL/dQ -----------------------------------------------------------------------------------------
         const float w = p.weights ? p.weights[r] : 1.0f;
-        float row = 0.f;
-#pragma unroll
-        for (int a = 0; a < kHeadMaxA; ++a) {
-            dq[a] = 0.f;
-            if (a < A) {
-                const float e = qo[a] - tgt[a];
-                float l, g;
-                if (p.huber) {
-                    const float ae = fabsf(e);
-                    const float qq = fminf(ae, 1.0f);
-                    l = 0.5f * qq * qq + (ae - qq);
-                    g = (ae <= 1.0f) ? e : (e > 0.f ? 1.0f : -1.0f);
-                } else {
-                    l = e * e;
-                    g = 2.0f * e;
-                }
-                row += l;
-                dq[a] = w * inv_b * g;
-            }
-        }
+        const float row = head_loss_grad(qo, tgt, A, p.huber, w, inv_b, dq);
         acc_loss += w * row;
         if (lane == 0) {
 #pragma unroll
@@ -275,30 +320,7 @@ __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadPar
 #pragma unroll
         for (int a = 0; a < kHeadMaxA; ++a) acc_b[a] += dq[a];
         __syncwarp();
-        // lane l now takes the KPL consecutive features [l KPL, (l + 1) KPL) of the row
-        float dz[KPL];
-#pragma unroll
-        for (int j = 0; j < KPL / 4; ++j) {
-            const float4 v = *reinterpret_cast<const float4*>(rowbuf + lane * KPL + 4 * j);
-            dz[4 * j] = v.x; dz[4 * j + 1] = v.y; dz[4 * j + 2] = v.z; dz[4 * j + 3] = v.w;
-        }
-        if (p.dh) {
-            float4* o = reinterpret_cast<float4*>(p.dh + (size_t)r * K + lane * KPL);
-#pragma unroll
-            for (int j = 0; j < KPL / 4; ++j) o[j] = make_float4(dz[4 * j], dz[4 * j + 1], dz[4 * j + 2], dz[4 * j + 3]);
-        }
-        if (p.dh_planes) {
-#pragma unroll
-            for (int c8 = 0; c8 < KPL / 8; ++c8) {
-                const float x8[8] = {dz[8 * c8], dz[8 * c8 + 1], dz[8 * c8 + 2], dz[8 * c8 + 3],
-                                     dz[8 * c8 + 4], dz[8 * c8 + 5], dz[8 * c8 + 6], dz[8 * c8 + 7]};
-                const HeadSplit8 sp = head_split8(x8);
-                uint16_t* d = p.dh_planes + head_tiled_elem((size_t)r, lane * KPL + 8 * c8, K);
-                *reinterpret_cast<uint4*>(d) = sp.h;
-                *reinterpret_cast<uint4*>(d + p.dh_plane_stride) = sp.m;
-                *reinterpret_cast<uint4*>(d + 2 * p.dh_plane_stride) = sp.l;
-            }
-        }
+        head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
     }
     // ---- per-warp partials: [dW (K * A) | db (A) | loss (1)] --------------------------------------------------------------
     float* part = p.workspace + (size_t)gw * ((size_t)K * A + A + 1);
@@ -333,6 +355,225 @@ __global__ void __launch_bounds__(256) dqn_head_reduce_kernel(const float* __res
         if (i < KA) dw[i] = s;
         else if (i < KA + A) db[i - KA] = s;
         else if (loss) *loss = s * inv_b;
+    }
+}
+
+// ---- fused Bootstrapped DQN ensemble head ---------------------------------------------------------------------------
+// H Q heads on one feature layer: head h owns the columns [h A, (h + 1) A) of one Dense(H A) kernel [K, H A]
+// (bootstrapped_dqn_agent.py:26-30).  Per head: Q of the three bindings, the double-DQN target of the head's own
+// selection where the sample's bootstrap mask is set (bootstrapped_dqn_agent.py:57-86; masked-out rows keep the online
+// prediction, so their dL/dQ is exactly 0), the head's loss (head.py:170-181) and its kernel / bias gradients.  The
+// gradient into the feature layer is r * sum_h dQ_h W_h^T, masked with relu'(h) (general_network.py:304-325: every head
+// copy reads (1 - r) stop_gradient(x) + r x).
+// Both networks' kernels of all heads do not fit in shared memory at H = 10, K = 512: the block stages one head at a
+// time and walks the heads in order; each warp accumulates its rows' sum over heads in its own shared-memory rows (lane
+// l owns features l + 32 j, as in head_dot), so no cross-block accumulation is needed and the bits are run-to-run
+// stable.  Per-head batch sums (dW, db, loss) leave through per-warp partials and a fixed-order second pass.
+struct EnsembleParams {
+    const float *h_next, *h_online, *h_select;
+    const float *w_target, *b_target, *w_online, *b_online;
+    const int64_t* actions;
+    const double* rewards;
+    const uint8_t* game_overs;
+    const uint8_t* masks;
+    double discount;
+    int huber, B, K, H, A;
+    float rescale;
+    float *q_online, *q_next, *q_select, *targets, *dq;
+    float* dh;
+    uint16_t* dh_planes;
+    int64_t dh_plane_stride;
+    float* workspace;
+};
+
+template <int KPL>
+__global__ void __launch_bounds__(32 * kHeadWarps) ensemble_head_fused_kernel(EnsembleParams p) {
+    // Wt_online [A][K] | Wt_target [A][K] of the current head | dz rows [warps][kHeadRows][K]
+    extern __shared__ __align__(16) float head_smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int gw = blockIdx.x * kHeadWarps + warp;
+    const int A = p.A, K = p.K, HA = p.H * p.A;
+    float* wt_on = head_smem;
+    float* wt_tg = head_smem + A * K;
+    float* dzrows = head_smem + 2 * A * K + warp * kHeadRows * K;
+#pragma unroll
+    for (int rr = 0; rr < kHeadRows; ++rr)
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) dzrows[rr * K + lane + 32 * j] = 0.f;
+    const float inv_b = 1.0f / (float)p.B;
+    const size_t per_head = (size_t)K * A + A + 1;
+    float* part = p.workspace + (size_t)gw * per_head * p.H;
+    for (int h = 0; h < p.H; ++h) {
+        __syncthreads();                                                  // the previous head's readers are done
+        for (int i = threadIdx.x; i < A * K; i += blockDim.x) {           // W[:, hA:(h+1)A] -> Wt [A][K]
+            const int k = i / A, a = i - k * A;
+            wt_on[a * K + k] = __ldg(p.w_online + (size_t)k * HA + h * A + a);
+            wt_tg[a * K + k] = __ldg(p.w_target + (size_t)k * HA + h * A + a);
+        }
+        __syncthreads();
+        float acc_w[KPL][kHeadMaxA];
+        float acc_b[kHeadMaxA], acc_loss = 0.f;
+#pragma unroll
+        for (int j = 0; j < KPL; ++j)
+#pragma unroll
+            for (int a = 0; a < kHeadMaxA; ++a) acc_w[j][a] = 0.f;
+#pragma unroll
+        for (int a = 0; a < kHeadMaxA; ++a) acc_b[a] = 0.f;
+#pragma unroll
+        for (int rr = 0; rr < kHeadRows; ++rr) {
+            const int r = gw * kHeadRows + rr;
+            if (r >= p.B) continue;
+            float hv[KPL], qn[kHeadMaxA], qs[kHeadMaxA], qo[kHeadMaxA];
+            head_dot<KPL>(p.h_next + (size_t)r * K, wt_tg, p.b_target + h * A, A, K, lane, hv, qn);
+            head_dot<KPL>(p.h_select + (size_t)r * K, wt_on, p.b_online + h * A, A, K, lane, hv, qs);
+            head_dot<KPL>(p.h_online + (size_t)r * K, wt_on, p.b_online + h * A, A, K, lane, hv, qo);
+            const bool use = p.masks[(size_t)r * p.H + h] != 0;
+            const float q_best = head_q_best(qs, qn, true, A);
+            const int64_t act = p.actions[r];
+            const double y = head_td_target(p.rewards[r], p.game_overs[r], p.discount, q_best);
+            float tgt[kHeadMaxA], dq[kHeadMaxA];
+#pragma unroll
+            for (int a = 0; a < kHeadMaxA; ++a) tgt[a] = (use && a < A && a == act) ? (float)y : qo[a];
+            acc_loss += head_loss_grad(qo, tgt, A, p.huber, 1.0f, inv_b, dq);
+            if (lane == 0) {
+                const size_t o = (size_t)r * HA + h * A;
+#pragma unroll
+                for (int a = 0; a < kHeadMaxA; ++a) {
+                    if (a < A) {
+                        p.q_online[o + a] = qo[a];
+                        if (p.q_next) p.q_next[o + a] = qn[a];
+                        if (p.q_select) p.q_select[o + a] = qs[a];
+                        p.targets[o + a] = tgt[a];
+                        p.dq[o + a] = dq[a];
+                    }
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < KPL; ++j) {
+                float s = 0.f;
+#pragma unroll
+                for (int a = 0; a < kHeadMaxA; ++a)
+                    if (a < A) {
+                        s = fmaf(dq[a], wt_on[a * K + lane + 32 * j], s);
+                        acc_w[j][a] = fmaf(hv[j], dq[a], acc_w[j][a]);
+                    }
+                dzrows[rr * K + lane + 32 * j] += s;
+            }
+#pragma unroll
+            for (int a = 0; a < kHeadMaxA; ++a) acc_b[a] += dq[a];
+        }
+        // per-warp partials of head h, head-major: [dW_h (K * A) | db_h (A) | loss_h (1)] -- the lanes' stores are as
+        // dense as dqn_head_fused_kernel's; the reduction scatters the sums into the [K, H A] kernel layout once
+        float* ph = part + (size_t)h * per_head;
+#pragma unroll
+        for (int j = 0; j < KPL; ++j)
+#pragma unroll
+            for (int a = 0; a < kHeadMaxA; ++a)
+                if (a < A) ph[((size_t)lane + 32 * j) * A + a] = acc_w[j][a];
+        if (lane == 0) {
+#pragma unroll
+            for (int a = 0; a < kHeadMaxA; ++a)
+                if (a < A) ph[(size_t)K * A + a] = acc_b[a];
+            ph[(size_t)K * A + A] = acc_loss;
+        }
+    }
+    // dL/dz = r * (sum over heads) * relu'(h), rescaled once in fp32 before the plane split
+#pragma unroll
+    for (int rr = 0; rr < kHeadRows; ++rr) {
+        const int r = gw * kHeadRows + rr;
+        if (r >= p.B) continue;
+        float* row = dzrows + rr * K;
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) {
+            const float hv = __ldg(p.h_online + (size_t)r * K + lane + 32 * j);
+            row[lane + 32 * j] = hv > 0.f ? __fmul_rn(p.rescale, row[lane + 32 * j]) : 0.f;
+        }
+        __syncwarp();
+        head_store_dz<KPL>(row, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+    }
+}
+
+// [nparts][H][K A + A + 1] partials -> dW [K, H A] | db [H A] | per-head losses, in the fixed order of
+// dqn_head_reduce_kernel
+__global__ void __launch_bounds__(256) ensemble_head_reduce_kernel(const float* __restrict__ ws, int nparts, int n_out,
+                                                                   int KA, int A, int HA, float inv_b,
+                                                                   float* __restrict__ dw, float* __restrict__ db,
+                                                                   float* __restrict__ losses) {
+    __shared__ float red[8][32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int i = blockIdx.x * 32 + lane;
+    float s = 0.f;
+    if (i < n_out)
+        for (int q = w; q < nparts; q += 8) s += ws[(size_t)q * n_out + i];
+    red[w][lane] = s;
+    __syncthreads();
+    if (w == 0 && i < n_out) {
+        for (int k = 1; k < 8; ++k) s += red[k][lane];
+        const int h = i / (KA + A + 1), j = i - h * (KA + A + 1);
+        if (j < KA) dw[(size_t)(j / A) * HA + h * A + j % A] = s;
+        else if (j < KA + A) db[h * A + j - KA] = s;
+        else losses[h] = s * inv_b;
+    }
+}
+// total loss = sum over the heads (general_network.py:352-360), in head order
+__global__ void ensemble_loss_total_kernel(const float* __restrict__ losses, int H, float* __restrict__ total) {
+    float s = losses[0];
+    for (int h = 1; h < H; ++h) s = __fadd_rn(s, losses[h]);
+    *total = s;
+}
+
+// ---- ensemble acting values: [E, H A] -> [E, A] ---------------------------------------------------------------------
+// the exploration policies' numpy arithmetic (exploration_policies/bootstrapped.py:70-84, ucb.py:70-83) in fp32 with
+// explicit rounding: numpy reduces axis 0 of a [H, A] array row after row, true-divides by H, and np.std squares the
+// deviations from that mean, sums them in the same order, divides by H and takes the square root
+__global__ void ensemble_action_values_kernel(const float* __restrict__ q, int E, int H, int A, int mode,
+                                              const int32_t* __restrict__ head, float lamb, float* __restrict__ out) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= E) return;
+    const float* qe = q + (size_t)e * H * A;
+    float* o = out + (size_t)e * A;
+    if (mode == CB200_ENSEMBLE_SELECT) {
+        const int h = head[e];
+        for (int a = 0; a < A; ++a) o[a] = qe[(size_t)h * A + a];
+        return;
+    }
+    if (mode == CB200_ENSEMBLE_VOTE) {
+        // np.argmax per head (first maximum), np.bincount, np.argmax of the counts (first maximum), one-hot
+        int best_c = 0, best_n = -1;
+        for (int c = 0; c < A; ++c) {
+            int n = 0;
+            for (int h = 0; h < H; ++h) {
+                const float* qh = qe + (size_t)h * A;
+                int am = 0;
+                for (int a = 1; a < A; ++a)
+                    if (qh[a] > qh[am]) am = a;
+                n += am == c;
+            }
+            if (n > best_n) {
+                best_n = n;
+                best_c = c;
+            }
+        }
+        for (int a = 0; a < A; ++a) o[a] = a == best_c ? 1.0f : 0.0f;
+        return;
+    }
+    const float fh = (float)H;
+    for (int a = 0; a < A; ++a) {
+        float s = qe[a];
+        for (int h = 1; h < H; ++h) s = __fadd_rn(s, qe[(size_t)h * A + a]);
+        const float mean = __fdiv_rn(s, fh);
+        if (mode == CB200_ENSEMBLE_MEAN) {
+            o[a] = mean;
+            continue;
+        }
+        const float d0 = __fsub_rn(qe[a], mean);
+        float ss = __fmul_rn(d0, d0);
+        for (int h = 1; h < H; ++h) {
+            const float d = __fsub_rn(qe[(size_t)h * A + a], mean);
+            ss = __fadd_rn(ss, __fmul_rn(d, d));
+        }
+        const float sd = __fsqrt_rn(__fdiv_rn(ss, fh));
+        o[a] = __fadd_rn(mean, __fmul_rn(lamb, sd));
     }
 }
 
@@ -530,6 +771,67 @@ int cb200_dqn_head_fused(const cb200_dqn_head_desc* d, void* stream) {
     const int n_out = p.K * p.A + p.A + 1;
     CB200_LAUNCH(dqn_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, p.workspace, nparts, n_out,
                  p.K * p.A, p.A, 1.0f / (float)p.B, p.dw, p.db, p.loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_ensemble_head_fused(const cb200_ensemble_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->h_next && d->h_online && d->h_select && d->w_target && d->b_target && d->w_online &&
+                        d->b_online && d->actions && d->rewards && d->game_overs && d->masks && d->q_online &&
+                        d->targets && d->dq && d->losses && d->dw && d->db && d->workspace,
+                    "null pointer");
+    CB200_CHECK_ARG(d->batch > 0 && d->batch <= (1 << 30), "bad batch");
+    CB200_CHECK_ARG(d->n_actions > 0 && d->n_actions <= kHeadMaxA, "1 <= n_actions <= 8");
+    CB200_CHECK_ARG(d->heads >= 1 && d->heads <= 64, "1 <= heads <= 64");
+    CB200_CHECK_ARG(d->features == 256 || d->features == 512, "features must be 256 or 512");
+    CB200_CHECK_ARG(!d->dh_planes || (d->dh_plane_stride % 8 == 0 && d->batch % 8 == 0), "planes: batch % 8, stride % 8");
+    EnsembleParams p;
+    p.h_next = d->h_next; p.h_online = d->h_online; p.h_select = d->h_select;
+    p.w_target = d->w_target; p.b_target = d->b_target; p.w_online = d->w_online; p.b_online = d->b_online;
+    p.actions = d->actions; p.rewards = d->rewards; p.game_overs = d->game_overs; p.masks = d->masks;
+    p.discount = d->discount; p.huber = d->huber; p.B = (int)d->batch; p.K = d->features; p.H = d->heads;
+    p.A = d->n_actions; p.rescale = d->grad_rescale;
+    p.q_online = d->q_online; p.q_next = d->q_next; p.q_select = d->q_select; p.targets = d->targets; p.dq = d->dq;
+    p.dh = d->dh; p.dh_planes = static_cast<uint16_t*>(d->dh_planes); p.dh_plane_stride = d->dh_plane_stride;
+    p.workspace = d->workspace;
+    const int warps = (p.B + kHeadRows - 1) / kHeadRows;
+    const unsigned grid = (unsigned)((warps + kHeadWarps - 1) / kHeadWarps);
+    const int nparts = (int)grid * kHeadWarps;
+    cudaStream_t st = as_stream(stream);
+    // <= 32 KB of staged head kernels + 32 KB of dz rows: above the 48 KB default, opted into once per instantiation
+    const size_t smem = (size_t)(2 * p.A * p.K + kHeadWarps * kHeadRows * p.K) * sizeof(float);
+    static bool attr_set[2] = {false, false};
+    const int ti = p.K == 512 ? 1 : 0;
+    if (!attr_set[ti]) {
+        if (ti)
+            CB200_CUDA(cudaFuncSetAttribute(ensemble_head_fused_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            64 * 1024));
+        else
+            CB200_CUDA(cudaFuncSetAttribute(ensemble_head_fused_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            64 * 1024));
+        attr_set[ti] = true;
+    }
+    if (p.K == 512) {
+        CB200_LAUNCH(ensemble_head_fused_kernel<16>, grid, 32 * kHeadWarps, smem, st, p);
+    } else {
+        CB200_LAUNCH(ensemble_head_fused_kernel<8>, grid, 32 * kHeadWarps, smem, st, p);
+    }
+    const int n_out = p.H * (p.K * p.A + p.A + 1);
+    CB200_LAUNCH(ensemble_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, p.workspace, nparts, n_out,
+                 p.K * p.A, p.A, p.H * p.A, 1.0f / (float)p.B, d->dw, d->db, d->losses);
+    if (d->loss) CB200_LAUNCH(ensemble_loss_total_kernel, 1, 1, 0, st, d->losses, p.H, d->loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_ensemble_action_values(const float* q, int64_t envs, int32_t heads, int32_t n_actions, int32_t mode,
+                                 const int32_t* head, float lamb, float* out, void* stream) {
+    CB200_CHECK_ARG(q && out && envs > 0 && envs <= (1 << 24) && heads >= 1 && n_actions >= 1, "bad arguments");
+    CB200_CHECK_ARG(mode >= CB200_ENSEMBLE_SELECT && mode <= CB200_ENSEMBLE_VOTE, "unknown mode");
+    CB200_CHECK_ARG(mode != CB200_ENSEMBLE_SELECT || head, "select mode needs the per-environment head indices");
+    CB200_LAUNCH(ensemble_action_values_kernel, (unsigned)((envs + 127) / 128), 128, 0, as_stream(stream), q, (int)envs,
+                 heads, n_actions, mode, head, lamb, out);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

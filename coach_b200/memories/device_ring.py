@@ -21,6 +21,7 @@ Columns
   ``action``     int64 scalar (discrete) or float vector (continuous), as given
   ``reward``     float64 (the reference's rewards are Python floats, core_types.py:523)
   ``game_over``  uint8
+  ``info:<key>`` ``transition.info[<key>]`` as declared (e.g. Bootstrapped DQN's ``info:mask``, uint8 [heads])
 """
 from collections import OrderedDict
 
@@ -250,8 +251,15 @@ class DeviceTransitionRing(object):
                 v = t.action
             elif name == "reward":
                 v = t.reward
-            else:
+            elif name == "game_over":
                 v = t.game_over
+            elif name.startswith("info:"):
+                if name[5:] not in t.info:
+                    raise ValueError("the replay stores column %r but the transition's info has no %r entry"
+                                     % (name, name[5:]))
+                v = t.info[name[5:]]
+            else:
+                raise ValueError("the replay stores column %r, which a Transition cannot supply" % name)
             a = np.asarray(v, dtype=sp.dtype, order='C')
             if a.shape != sp.shape:
                 raise ValueError("transition field %s has shape %s, the replay was created with %s"

@@ -409,6 +409,63 @@ typedef struct cb200_dqn_head_desc {
 
 int cb200_dqn_head_fused(const cb200_dqn_head_desc* h_desc, void* stream);
 
+/* Fused Bootstrapped DQN ensemble head (agents/bootstrapped_dqn_agent.py:26-30,57-86): `heads` Q heads on one feature
+ * layer, head h owning the columns [h n_actions, (h + 1) n_actions) of one kernel [features, heads * n_actions].  Per
+ * head and sample where masks[i, h] != 0: a* = argmax of the online head on s', target = r + (1 - done) * discount *
+ * Q_target_h(s', a*) (fp64, bit-exact given the Q values, as cb200_dqn_head_fused); elsewhere the target is the online
+ * prediction, so dL/dQ is exactly 0.  Per-head Huber / MSE loss mean_b(sum_a l) (heads/head.py:170-181), their sum,
+ * dL/dQ, the head kernel's gradients, and the gradient w.r.t. the feature layer's pre-activation
+ * grad_rescale * sum_h dQ_h W_h^T masked with relu'(h) (general_network.py:304-325), rescaled in fp32 before it is split
+ * into operand planes.  features 256 or 512, n_actions <= 8, heads <= 64.  Deterministic: no atomics. */
+typedef struct cb200_ensemble_head_desc {
+    const float* h_next;        /* [batch, features] post-ReLU features of s' from the TARGET network                      */
+    const float* h_online;      /* [batch, features] features of s from the online network                                */
+    const float* h_select;      /* [batch, features] features of s' from the online network (per-head action selection)   */
+    const float* w_target;      /* target head kernel [features, heads * n_actions] and bias [heads * n_actions]           */
+    const float* b_target;
+    const float* w_online;
+    const float* b_online;
+    const int64_t* actions;     /* [batch]                                                                                 */
+    const double* rewards;
+    const uint8_t* game_overs;
+    const uint8_t* masks;       /* [batch, heads] bootstrap masks                                                          */
+    double discount;
+    int32_t huber;              /* 1: tf.losses.huber_loss(delta 1), 0: mean squared error                                */
+    int64_t batch;
+    int32_t features;           /* 256 or 512                                                                              */
+    int32_t heads;              /* 1 .. 64                                                                                 */
+    int32_t n_actions;          /* per head, <= 8                                                                          */
+    float grad_rescale;         /* r of general_network.py:304-325                                                        */
+    float* q_online;            /* out [batch, heads * n_actions]                                                          */
+    float* q_next;              /* out, optional                                                                           */
+    float* q_select;            /* out, optional                                                                           */
+    float* targets;             /* out [batch, heads * n_actions]                                                          */
+    float* dq;                  /* out [batch, heads * n_actions]: dL/dQ                                                   */
+    float* losses;              /* out [heads]: per-head loss                                                              */
+    float* loss;                /* out scalar, optional: sum of the per-head losses                                        */
+    float* dh;                  /* out, optional: [batch, features] dL/d(pre-activation of the feature layer)             */
+    void* dh_planes;            /* out, optional: the same as tiled bf16 hi / mid / lo planes                              */
+    int64_t dh_plane_stride;
+    float* dw;                  /* out [features, heads * n_actions]                                                       */
+    float* db;                  /* out [heads * n_actions]                                                                 */
+    float* workspace;           /* ceil(batch / 16) * 8 * ((features + 1) * heads * n_actions + heads) floats             */
+} cb200_ensemble_head_desc;
+
+int cb200_ensemble_head_fused(const cb200_ensemble_head_desc* e_desc, void* stream);
+
+/* Acting values of an ensemble, q [envs, heads * n_actions] -> out [envs, n_actions], in the exploration policies' fp32
+ * numpy arithmetic (exploration_policies/bootstrapped.py:70-84, ucb.py:70-83):
+ *   SELECT  the row of head[e] (Bootstrapped, training)
+ *   UCB     mean + lamb * std over the heads, population std (UCB, training)
+ *   MEAN    mean over the heads (UCB, evaluation)
+ *   VOTE    one-hot of the majority vote of the heads' argmaxes, ties to the lowest action (Bootstrapped, evaluation) */
+#define CB200_ENSEMBLE_SELECT 0
+#define CB200_ENSEMBLE_UCB 1
+#define CB200_ENSEMBLE_MEAN 2
+#define CB200_ENSEMBLE_VOTE 3
+int cb200_ensemble_action_values(const float* q, int64_t envs, int32_t heads, int32_t n_actions, int32_t mode,
+                                 const int32_t* head, float lamb, float* out, void* stream);
+
 /* DuelingQHead (heads/dueling_q_head.py:33-47): q = v + (adv - mean_a adv); backward: d_v = sum_a dq,
  * d_adv = dq - mean_a dq. */
 int cb200_dueling_combine_fwd(const float* v, const float* adv, int64_t batch, int64_t n_actions, float* q,
