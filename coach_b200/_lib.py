@@ -60,7 +60,14 @@ class DqnHeadDesc(ctypes.Structure):
                 ("huber", ctypes.c_int32), ("batch", c_i64), ("features", ctypes.c_int32),
                 ("n_actions", ctypes.c_int32), ("q_online", c_void_p), ("q_next", c_void_p), ("targets", c_void_p),
                 ("td_err", c_void_p), ("dq", c_void_p), ("loss", c_void_p), ("dh", c_void_p), ("dh_planes", c_void_p),
-                ("dh_plane_stride", c_i64), ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p)]
+                ("dh_plane_stride", c_i64), ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p),
+                ("target_rule", ctypes.c_int32), ("h_target_s", c_void_p), ("mc_returns", c_void_p),
+                ("pal_alpha", c_double), ("mc_mixing_rate", c_double), ("q_select", c_void_p),
+                ("q_target_s", c_void_p)]
+
+
+# cb200_dqn_head_desc.target_rule
+TARGET_DQN, TARGET_MMC, TARGET_PAL, TARGET_PAL_PERSISTENT = 0, 1, 2, 3
 
 
 class EnsembleHeadDesc(ctypes.Structure):

@@ -69,11 +69,11 @@ class DDQNAgentParameters(DQNAgentParameters):
 
 
 class QNetworkWrapper(object):
-    """online + target parameter buffers over one QNetworkDef (network_wrapper.py:31-116), with the three forward
-    bindings a DQN step needs: online(s) [training], target(s'), online(s') [DDQN]."""
+    """online + target parameter buffers over one QNetworkDef (network_wrapper.py:31-116), with the forward bindings a
+    DQN step needs: online(s) [training], target(s'), online(s') [DDQN], target(s) [PAL: ``target_s``]."""
 
     def __init__(self, lib, net_def, params: NetworkParameters, batch_size, batch_buffers, double_dqn, device,
-                 input_planes=None):
+                 input_planes=None, target_s=False):
         self.lib, self.net, self.params, self.B = lib, net_def, params, batch_size
         self.store = net_def.store
         self.ws = Workspace(device)
@@ -87,6 +87,9 @@ class QNetworkWrapper(object):
         self.target_s2 = net_def.instantiate(lib, self.ws_target, batch_size, s2, self.theta_target) \
             if self.theta_target is not None else None
         self.online_s2 = net_def.instantiate(lib, self.ws, batch_size, s2, self.theta) if double_dqn else None
+        # the target network over the same input as online_s (on the fused input path: the same s2d plane)
+        self.target_s = net_def.instantiate(lib, self.ws_target, batch_size, s, self.theta_target) \
+            if target_s and self.theta_target is not None else None
         self.sumsq = torch.zeros(1, dtype=torch.float32, device=device)
         self.has_target = self.theta_target is not None
         # Adam state: the fp32 running powers of TF's non-slot beta1 / beta2 power variables, kept on the device
@@ -97,7 +100,7 @@ class QNetworkWrapper(object):
         # parameter planes (operands of the tensor-core GEMMs) are re-derived where the parameters are written, not in
         # every forward pass: the target network's once per target update instead of once per learn step
         self._planes = []
-        for inst in (self.online_s, self.online_s2, self.target_s2):
+        for inst in (self.online_s, self.online_s2, self.target_s2, self.target_s):
             self.add_planes(inst)
 
     def add_planes(self, inst):
@@ -150,6 +153,7 @@ class QNetworkWrapper(object):
 
 class DQNAgent(object):
     double_dqn = False
+    target_on_s = False        # PAL: the target network's Q values on s (QNetworkWrapper.target_s)
 
     def __init__(self, agent_parameters, parent=None, observation_shape=None, num_actions=None, device=None,
                  seed=None):
@@ -180,8 +184,10 @@ class DQNAgent(object):
         }
         extra = self._extra_columns()
         self.batch_buffers.update(extra)
+        derived = self._memory_columns()
+        self.batch_buffers.update(derived)
         # columns whose persistent buffers a batch must use for the CUDA-graph replay (fixed pointers in the graphs)
-        self._own_columns = ("action", "reward", "game_over") + tuple(extra)
+        self._own_columns = ("action", "reward", "game_over") + tuple(extra) + tuple(derived)
         # the ring's column layout = the agent's batch buffers, fixed before the first store: store(Transition) then
         # casts what the environment hands out (gym: float64) instead of the gather overrunning float32 buffers
         if hasattr(self.memory, "declare_schema") and self.memory.ring.specs is None:
@@ -211,7 +217,8 @@ class DQNAgent(object):
                         "geometry": (H, W, C, S)}
         self.networks = {"main": QNetworkWrapper(self.lib, self.net_def, net_params, B, self.batch_buffers,
                                                  self.double_dqn, dev,
-                                                 input_planes=self.s2d["columns"] if self.s2d else None)}
+                                                 input_planes=self.s2d["columns"] if self.s2d else None,
+                                                 target_s=self.target_on_s)}
         if self.networks["main"].has_target:
             self.networks["main"].sync()
         # plain Q head: head forward passes, TD targets, loss and the head's backward pass are ONE fused launch
@@ -270,9 +277,16 @@ class DQNAgent(object):
         bootstrap masks); they join the ring's schema and the own-buffer check of the CUDA-graph replay"""
         return {}
 
+    def _memory_columns(self):
+        """batch columns the memory derives itself rather than storing them (MMC / PAL: the episodic replay's Monte
+        Carlo returns), as {name: persistent batch buffer}: sampled into and part of the own-buffer check of the
+        CUDA-graph replay, but not ring columns"""
+        return {}
+
     def _head_fusable(self, net):
         return (net.online_s.head_fusable() and net.target_s2.head_fusable() and
-                (net.online_s2 is None or net.online_s2.head_fusable()))
+                (net.online_s2 is None or net.online_s2.head_fusable()) and
+                (net.target_s is None or net.target_s.head_fusable()))
 
     # ---- reference plumbing ------------------------------------------------------------------------------------------
     @property
@@ -332,6 +346,8 @@ class DQNAgent(object):
             d.dh_planes, d.dh_plane_stride = pl.ptr, pl.stride
         d.dw, d.db = store.view(store.grad, wname).data_ptr(), store.view(store.grad, bname).data_ptr()
         d.workspace = self._head_keep[0].data_ptr()
+        # descriptor field -> batch column, pointed at the step's batch before every head launch
+        self._head_columns = {"actions": "action", "rewards": "reward", "game_overs": "game_over"}
         self.head_desc = d
 
     # ---- acting path (SURVEY.md 8f-4) --------------------------------------------------------------------------------
@@ -382,12 +398,14 @@ class DQNAgent(object):
             d = self.head_desc
             with self._side_fwd:
                 net.target_s2.forward_features()
+                if net.target_s is not None:
+                    net.target_s.forward_features()
             net.online_s.forward_features()
             if self.double_dqn:
                 net.online_s2.forward_features()
             self._side_fwd.join()
-            d.actions, d.rewards, d.game_overs = cols["action"].data_ptr(), cols["reward"].data_ptr(), \
-                cols["game_over"].data_ptr()
+            for field, name in self._head_columns.items():
+                setattr(d, field, cols[name].data_ptr())
             d.weights = self._head_weights.data_ptr() if self._head_weights is not None else None
             d.targets, d.td_err, d.loss = self.targets.data_ptr(), self.td_err.data_ptr(), self.loss_dev.data_ptr()
             _lib.check(lib.cb200_dqn_head_fused(ctypes.byref(d), st))

@@ -140,6 +140,11 @@ struct HeadParams {
     uint16_t* dh_planes;
     int64_t dh_plane_stride;
     float *dw, *db, *workspace;
+    // target rules beyond DQN / DDQN (appended: the DQN rule reads nothing below)
+    const float* h_target_s;
+    const double* mc_returns;
+    double pal_alpha, mc_mixing_rate;
+    float *q_select, *q_target_s;
 };
 
 // Lane l owns features k = l + 32 j (j < KPL): a row of h is read with coalesced 128-byte loads and the head kernels,
@@ -187,6 +192,40 @@ __device__ __forceinline__ double head_td_target(double reward, uint8_t game_ove
     const double not_done = __dsub_rn(1.0, game_over ? 1.0 : 0.0);
     return __dadd_rn(reward, __dmul_rn(__dmul_rn(not_done, discount), (double)q_best));
 }
+// the fp32 target of the taken action under a target rule, given the double-DQN target y (fp64, head_td_target), the
+// target head's Q values on s' (qn) and on s (qt, PAL only), q_best = qn[a*], and the sample's Monte Carlo return R.
+// Every operation is an explicit _rn intrinsic: the reference's numpy rounding order, nothing FMA-contracted.
+template <int RULE>
+__device__ __forceinline__ float head_rule_target(double y, float q_best, const float (&qn)[kHeadMaxA],
+                                                  const float (&qt)[kHeadMaxA], int64_t act, int A, double R,
+                                                  double alpha, double rho) {
+    if constexpr (RULE == CB200_TARGET_DQN) {
+        return (float)y;                                                  // dqn_agent.py:103 (fp32 element assignment)
+    } else if constexpr (RULE == CB200_TARGET_MMC) {
+        // mmc_agent.py:72-78: (1 - rho) * one_step_target + rho * monte_carlo_target, all fp64, then stored as fp32
+        return (float)__dadd_rn(__dmul_rn(__dsub_rn(1.0, rho), y), __dmul_rn(rho, R));
+    } else {
+        // pal_agent.py:83-106: every statement writes into the float32 TD_targets array (numpy 2 scalar promotion)
+        float vt = qt[0], vn = qn[0], qta = qt[0];
+#pragma unroll
+        for (int a = 1; a < kHeadMaxA; ++a) {
+            if (a < A) {
+                vt = qt[a] > vt ? qt[a] : vt;                             // np.max(q_st_target, 1)
+                vn = qn[a] > vn ? qn[a] : vn;                             // np.max(q_st_plus_1_target, 1)
+                if (a == act) qta = qt[a];
+            }
+        }
+        const float t0 = (float)y;
+        const float adv = __fsub_rn(vt, qta);                             // advantage_learning_update
+        const float nadv = __fsub_rn(vn, q_best);                         // next_advantage_learning_update
+        // Python's min(adv, nadv): the first argument unless the second is strictly smaller
+        const float m = (RULE == CB200_TARGET_PAL_PERSISTENT && nadv < adv) ? nadv : adv;
+        const float t1 = __fsub_rn(t0, __fmul_rn((float)alpha, m));       // -= alpha * m (alpha demoted to fp32)
+        const float t2 = __fmul_rn((float)__dsub_rn(1.0, rho), t1);       // (1 - rho) * t, 1 - rho in fp64 then demoted
+        return (float)__dadd_rn((double)t2, __dmul_rn(rho, R));           // + rho * R: fp32 + fp64 -> fp64
+    }
+}
+
 // head loss of one row and dL/dQ (head.py:165-177; tf.losses.huber_loss delta = 1 / mean_squared_error)
 __device__ __forceinline__ float head_loss_grad(const float (&qo)[kHeadMaxA], const float (&tgt)[kHeadMaxA], int A,
                                                 int huber, float w, float inv_b, float (&dq)[kHeadMaxA]) {
@@ -242,8 +281,11 @@ __device__ __forceinline__ void head_store_dz(const float* rowbuf, int lane, int
     }
 }
 
-template <int KPL>
+// RULE: CB200_TARGET_* (the target of the taken action; see head_rule_target).  PAL adds one head_dot, the target
+// head on h_target_s; the loss, dL/dQ and the backward pass are the same for every rule.
+template <int KPL, int RULE>
 __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadParams p) {
+    constexpr bool kPal = RULE == CB200_TARGET_PAL || RULE == CB200_TARGET_PAL_PERSISTENT;
     extern __shared__ __align__(16) float head_smem[];     // Wt_online [A][K] | Wt_target [A][K] | row buffers [warps][K]
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int gw = blockIdx.x * kHeadWarps + warp;                        // global warp
@@ -270,9 +312,10 @@ __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadPar
     for (int rr = 0; rr < kHeadRows; ++rr) {
         const int r = gw * kHeadRows + rr;
         if (r >= p.B) break;
-        float hv[KPL], qn[kHeadMaxA], qs[kHeadMaxA], qo[kHeadMaxA];
+        float hv[KPL], qn[kHeadMaxA], qs[kHeadMaxA], qo[kHeadMaxA], qt[kHeadMaxA];
         head_dot<KPL>(p.h_next + (size_t)r * K, wt_tg, p.b_target, A, K, lane, hv, qn);
         if (use_sel) head_dot<KPL>(p.h_select + (size_t)r * K, wt_on, p.b_online, A, K, lane, hv, qs);
+        if constexpr (kPal) head_dot<KPL>(p.h_target_s + (size_t)r * K, wt_tg, p.b_target, A, K, lane, hv, qt);
         head_dot<KPL>(p.h_online + (size_t)r * K, wt_on, p.b_online, A, K, lane, hv, qo);    // hv = h_online slice
         // ---- TD target (every lane, identical values) -- dqn_agent.py:92-103 ------------------------------------------
         const float q_best = head_q_best(qs, qn, use_sel, A);
@@ -280,12 +323,27 @@ __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadPar
         const double y = head_td_target(p.rewards[r], p.game_overs[r], p.discount, q_best);
         float tgt[kHeadMaxA], dq[kHeadMaxA];
         double td = 0.0;
+        if constexpr (RULE == CB200_TARGET_DQN) {
 #pragma unroll
-        for (int a = 0; a < kHeadMaxA; ++a) {
-            tgt[a] = qo[a];
-            if (a < A && a == act) {
-                td = fabs(__dsub_rn(y, (double)qo[a]));
-                tgt[a] = (float)y;
+            for (int a = 0; a < kHeadMaxA; ++a) {
+                tgt[a] = qo[a];
+                if (a < A && a == act) {
+                    td = fabs(__dsub_rn(y, (double)qo[a]));
+                    tgt[a] = (float)y;
+                }
+            }
+        } else {
+            const bool in_range = act >= 0 && act < A;
+            const float ty = in_range ? head_rule_target<RULE>(y, q_best, qn, qt, act, A, p.mc_returns[r], p.pal_alpha,
+                                                               p.mc_mixing_rate)
+                                      : 0.f;
+#pragma unroll
+            for (int a = 0; a < kHeadMaxA; ++a) {
+                tgt[a] = qo[a];
+                if (a < A && a == act) {
+                    td = fabs(__dsub_rn((double)ty, (double)qo[a]));
+                    tgt[a] = ty;
+                }
             }
         }
         // ---- head loss and dL/dQ -----------------------------------------------------------------------------------------
@@ -300,6 +358,10 @@ __global__ void __launch_bounds__(32 * kHeadWarps) dqn_head_fused_kernel(HeadPar
                     if (p.q_next) p.q_next[(size_t)r * A + a] = qn[a];
                     p.targets[(size_t)r * A + a] = tgt[a];
                     p.dq[(size_t)r * A + a] = dq[a];
+                    if constexpr (RULE != CB200_TARGET_DQN) {
+                        if (p.q_select) p.q_select[(size_t)r * A + a] = qs[a];
+                        if (kPal && p.q_target_s) p.q_target_s[(size_t)r * A + a] = qt[a];
+                    }
                 }
             }
             p.td_err[r] = td;
@@ -749,6 +811,11 @@ int cb200_dqn_head_fused(const cb200_dqn_head_desc* d, void* stream) {
     CB200_CHECK_ARG(d->batch > 0 && d->n_actions > 0 && d->n_actions <= kHeadMaxA, "1 <= n_actions <= 8");
     CB200_CHECK_ARG(d->features == 256 || d->features == 512, "features must be 256 or 512");
     CB200_CHECK_ARG(!d->dh_planes || (d->dh_plane_stride % 8 == 0 && d->batch % 8 == 0), "planes: batch % 8, stride % 8");
+    const int rule = d->target_rule;
+    CB200_CHECK_ARG(rule >= CB200_TARGET_DQN && rule <= CB200_TARGET_PAL_PERSISTENT, "unknown target rule");
+    CB200_CHECK_ARG(rule == CB200_TARGET_DQN || (d->h_select && d->mc_returns),
+                    "MMC / PAL targets need h_select and mc_returns");
+    CB200_CHECK_ARG(rule < CB200_TARGET_PAL || d->h_target_s, "PAL targets need h_target_s");
     HeadParams p;
     p.h_next = d->h_next; p.h_online = d->h_online; p.h_select = d->h_select;
     p.w_target = d->w_target; p.b_target = d->b_target; p.w_online = d->w_online; p.b_online = d->b_online;
@@ -758,16 +825,27 @@ int cb200_dqn_head_fused(const cb200_dqn_head_desc* d, void* stream) {
     p.dq = d->dq; p.loss = d->loss; p.dh = d->dh;
     p.dh_planes = static_cast<uint16_t*>(d->dh_planes); p.dh_plane_stride = d->dh_plane_stride;
     p.dw = d->dw; p.db = d->db; p.workspace = d->workspace;
+    p.h_target_s = d->h_target_s; p.mc_returns = d->mc_returns;
+    p.pal_alpha = d->pal_alpha; p.mc_mixing_rate = d->mc_mixing_rate;
+    p.q_select = d->q_select; p.q_target_s = d->q_target_s;
     const int warps = (p.B + kHeadRows - 1) / kHeadRows;
     const unsigned grid = (unsigned)((warps + kHeadWarps - 1) / kHeadWarps);
     const int nparts = (int)grid * kHeadWarps;                 // idle warps of the last block write zero partials
     cudaStream_t st = as_stream(stream);
     const size_t smem = (size_t)(2 * p.A * p.K + kHeadWarps * p.K) * sizeof(float);      // <= 48 KB (A <= 8, K <= 512)
-    if (p.K == 512) {
-        CB200_LAUNCH(dqn_head_fused_kernel<16>, grid, 32 * kHeadWarps, smem, st, p);
-    } else {
-        CB200_LAUNCH(dqn_head_fused_kernel<8>, grid, 32 * kHeadWarps, smem, st, p);
+#define CB200_HEAD_LAUNCH(R)                                                                \
+    if (p.K == 512) {                                                                       \
+        CB200_LAUNCH((dqn_head_fused_kernel<16, R>), grid, 32 * kHeadWarps, smem, st, p);   \
+    } else {                                                                                \
+        CB200_LAUNCH((dqn_head_fused_kernel<8, R>), grid, 32 * kHeadWarps, smem, st, p);    \
     }
+    switch (rule) {
+        case CB200_TARGET_MMC: CB200_HEAD_LAUNCH(CB200_TARGET_MMC); break;
+        case CB200_TARGET_PAL: CB200_HEAD_LAUNCH(CB200_TARGET_PAL); break;
+        case CB200_TARGET_PAL_PERSISTENT: CB200_HEAD_LAUNCH(CB200_TARGET_PAL_PERSISTENT); break;
+        default: CB200_HEAD_LAUNCH(CB200_TARGET_DQN); break;
+    }
+#undef CB200_HEAD_LAUNCH
     const int n_out = p.K * p.A + p.A + 1;
     CB200_LAUNCH(dqn_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, p.workspace, nparts, n_out,
                  p.K * p.A, p.A, 1.0f / (float)p.B, p.dw, p.db, p.loss);

@@ -27,6 +27,8 @@ class EpisodicExperienceReplayParameters(MemoryParameters):
         self.max_size = (MemoryGranularity.Transitions, 1000000)
         self.n_step = -1
         self.train_to_eval_ratio = 1
+        # coach_b200 only: the ring's size in transitions when max_size counts episodes
+        self.transition_capacity = None
 
     @property
     def path(self):
@@ -34,11 +36,25 @@ class EpisodicExperienceReplayParameters(MemoryParameters):
 
 
 class EpisodicExperienceReplay(ExperienceReplay):
+    """``max_size`` in transitions sizes the ring; in episodes (``MemoryGranularity.Episodes``) it caps the number of
+    listed episodes and ``transition_capacity`` sizes the ring, which must then hold every listed episode: a store that
+    would overwrite a slot of one raises ``ValueError``."""
+
     def __init__(self, max_size: Tuple[MemoryGranularity, int] = (MemoryGranularity.Transitions, 1000000),
-                 n_step=-1, train_to_eval_ratio: int = 1, discount: float = 0.99, device=None):
-        if max_size[0] != MemoryGranularity.Transitions:
-            raise ValueError("the HBM-resident episodic replay is sized in transitions")
-        ExperienceReplay.__init__(self, max_size, True, device=device)
+                 n_step=-1, train_to_eval_ratio: int = 1, discount: float = 0.99, device=None,
+                 transition_capacity: int = None):
+        if max_size[0] == MemoryGranularity.Episodes:
+            if transition_capacity is None:
+                raise ValueError("an episode-sized replay needs transition_capacity: the ring is sized in transitions")
+            if max_size[1] < 1:
+                raise ValueError("an episode-sized replay holds at least one episode")
+            ExperienceReplay.__init__(self, (MemoryGranularity.Transitions, int(transition_capacity)), True,
+                                      device=device)
+            self.max_size = max_size
+        elif max_size[0] == MemoryGranularity.Transitions:
+            ExperienceReplay.__init__(self, max_size, True, device=device)
+        else:
+            raise ValueError("max_size is counted in transitions or episodes")
         self.n_step = n_step
         self.discount = discount
         self.episode_lengths = []          # complete episodes, oldest first
@@ -48,7 +64,10 @@ class EpisodicExperienceReplay(ExperienceReplay):
 
     # ---- counters (episodic_experience_replay.py:75-100) -----------------------------------------------------------
     def length(self, lock: bool = False) -> int:
-        """number of episodes, counting the open one like the reference's buffer list"""
+        """number of episodes, counting the open one like the reference's buffer list -- except that an episode-sized
+        replay counts it only when it is non-empty, as the reference's length() does (:77-85)"""
+        if self.max_size[0] == MemoryGranularity.Episodes:
+            return len(self.episode_lengths) + (1 if self._open_len > 0 else 0)
         return len(self.episode_lengths) + 1
 
     def num_complete_episodes(self):
@@ -64,7 +83,15 @@ class EpisodicExperienceReplay(ExperienceReplay):
     def _evict(self):
         """_enforce_max_length (:215-228, Transitions granularity): whole oldest episodes go while the buffer holds
         more transitions than max_size -- checked at every store, like the reference, so the ring (capacity =
-        max_size slots) never overwrites a slot of an episode that is still listed"""
+        max_size slots) never overwrites a slot of an episode that is still listed.  Episodes granularity: whole oldest
+        episodes go while length() exceeds max_size; listed episodes that outgrow the ring raise."""
+        if self.max_size[0] == MemoryGranularity.Episodes:
+            while self.episode_lengths and self.length() > self.max_size[1]:
+                self.episode_lengths.pop(0)
+            if sum(self.episode_lengths) + self._open_len > self.ring.capacity:
+                raise ValueError("the listed episodes need more than the ring's %d transitions (transition_capacity)"
+                                 % self.ring.capacity)
+            return
         while self.episode_lengths and sum(self.episode_lengths) + self._open_len > self.ring.capacity:
             self.episode_lengths.pop(0)
         if self._open_len > self.ring.capacity:
@@ -215,19 +242,26 @@ class EpisodicExperienceReplay(ExperienceReplay):
     def get(self, episode_index: int, lock: bool = True):
         return self.get_episode(episode_index, lock)
 
-    def sample_batch(self, size: int, out: dict = None) -> DeviceBatch:
-        """episodic_experience_replay.py:102-130: uniform over the transitions of complete episodes."""
+    def sample_batch(self, size: int, out: dict = None, s2d: dict = None) -> DeviceBatch:
+        """episodic_experience_replay.py:102-130: uniform over the transitions of complete episodes.  The batch carries
+        their Monte Carlo returns as ``n_step_discounted_rewards`` (fp64), written into ``out[...]`` when ``out`` has
+        that buffer.  ``s2d``: image columns as space-to-depth operand planes (ExperienceReplay.sample_batch)."""
         n = self.num_transitions_in_complete_episodes()
         if n < 1:
             raise ValueError("The episodic replay buffer cannot be sampled since there are no complete episodes yet. "
                              "There is currently 1 episodes with {} transitions".format(self._open_len))
         self._flush()
         pos = np.random.randint(n, size=size)                                   # :121
-        slots = self._slots_of_complete_episodes(pos)       # only the drawn positions: no O(buffer) host work per step
-        idx = torch.from_numpy(slots).to(self.device)
-        cols = dict(self.ring.gather(idx, out))
-        cols["idx"] = idx
-        return DeviceBatch(cols, size)
+        # only the drawn positions are mapped to slots: no O(buffer) host work per step
+        batch = self._gather_slots(self._slots_of_complete_episodes(pos), size, out, s2d)
+        idx = batch.columns["idx"]
+        ret = out.get("n_step_discounted_rewards") if out is not None else None
+        if ret is not None:
+            torch.index_select(self._returns, 0, idx, out=ret)
+        else:
+            ret = self._returns[idx]
+        batch.columns["n_step_discounted_rewards"] = ret
+        return batch
 
     def clean(self, lock: bool = True) -> None:
         self.assert_not_frozen()

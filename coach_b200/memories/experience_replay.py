@@ -121,7 +121,12 @@ class ExperienceReplay(Memory):
         ``s2d``: image columns as space-to-depth operand planes (see PrioritizedExperienceReplay.sample_batch)."""
         pos = self._draw_positions(size)
         self._flush()
-        slots = torch.from_numpy(self._positions_to_slots(pos).astype(np.int64))
+        return self._gather_slots(self._positions_to_slots(pos), size, out, s2d)
+
+    def _gather_slots(self, slots: np.ndarray, size: int, out: dict = None, s2d: dict = None) -> DeviceBatch:
+        """the rows of the given ring slots as a DeviceBatch: into ``out`` (persistent buffers) or fresh tensors, the
+        image columns optionally as space-to-depth operand planes (``s2d``)"""
+        slots = torch.from_numpy(np.asarray(slots).astype(np.int64))
         idx = slots.pin_memory().to(self.device, non_blocking=True) if self.device.type == "cuda" else slots
         if s2d is not None:
             from coach_b200.memories.prioritized_experience_replay import _LazyColumns

@@ -405,7 +405,27 @@ typedef struct cb200_dqn_head_desc {
     float* dw;                  /* out [features, n_actions]: gradient of the online head kernel                          */
     float* db;                  /* out [n_actions]                                                                         */
     float* workspace;           /* ceil(batch / 16) * 8 * (features * n_actions + n_actions + 1) floats                    */
+    /* Target rule of the taken action (CB200_TARGET_*); a zero-initialised tail means DQN / DDQN.  Every rule selects
+     * a* = argmax Q_online(s') (first maximum; h_select required) and starts from the fp64 double-DQN target
+     * y = r + ((1 - done) discount) Q_target(s')[a*], bit-exact given the Q values:
+     *   MMC (mmc_agent.py:63-78):  target = (float)((1 - rho) y + rho R), fp64, R = mc_returns[i]
+     *   PAL (pal_agent.py:70-106): t0 = (float)y; adv = max Qt(s) - Qt(s)[a]; nadv = max Qt(s') - Qt(s')[a*];
+     *     m = adv (PAL) or min(adv, nadv) (persistent: nadv only when strictly smaller); t1 = t0 - (float)alpha m;
+     *     t2 = (float)(1 - rho) t1; target = (float)((double)t2 + rho R) -- fp32 steps, as numpy evaluates them.
+     * td_err is |target - Q(s, a)| of the final target for these rules. */
+    int32_t target_rule;
+    const float* h_target_s;    /* PAL: [batch, features] features of s from the TARGET network                            */
+    const double* mc_returns;   /* MMC / PAL: [batch] Monte Carlo returns (the replay's n_step_discounted_rewards)         */
+    double pal_alpha;
+    double mc_mixing_rate;      /* rho                                                                                     */
+    float* q_select;            /* out, optional (MMC / PAL): [batch, n_actions] Q_online(s')                              */
+    float* q_target_s;          /* out, optional (PAL): [batch, n_actions] Q_target(s)                                     */
 } cb200_dqn_head_desc;
+
+#define CB200_TARGET_DQN 0
+#define CB200_TARGET_MMC 1
+#define CB200_TARGET_PAL 2
+#define CB200_TARGET_PAL_PERSISTENT 3
 
 int cb200_dqn_head_fused(const cb200_dqn_head_desc* h_desc, void* stream);
 
