@@ -48,10 +48,18 @@ class CategoricalDQNAgent(DQNAgent):
     double_q_selection = False       # RainbowDQNAgent's rule: the online network picks the target action
 
     def __init__(self, agent_parameters, parent=None, **kwargs):
+        alg = agent_parameters.algorithm
+        z = np.linspace(alg.v_min, alg.v_max, alg.atoms)                                     # categorical_dqn_agent.py:77
+        top = (z[-1] - z[0]) / (z[1] - z[0])
+        if top > alg.atoms - 1:
+            raise ValueError(
+                "CategoricalDQNAgent: the support linspace(%r, %r, %d) puts v_max at bin position %r > %d; the reference "
+                "agent raises IndexError on the first sample whose projected target reaches v_max" %
+                (alg.v_min, alg.v_max, alg.atoms, float(top), alg.atoms - 1))
         super().__init__(agent_parameters, parent, **kwargs)
         alg = self.ap.algorithm
         B, A, N, dev = self.batch_size, self.num_actions, int(alg.atoms), self.device
-        self.z_values = np.linspace(alg.v_min, alg.v_max, alg.atoms)                         # categorical_dqn_agent.py:77
+        self.z_values = z
         self._z = torch.from_numpy(self.z_values).to(dev)
         # the head's own support: float32 constant cast to float64 (categorical_q_head.py:36-37)
         self._z_head = torch.from_numpy(self.z_values.astype(np.float32).astype(np.float64)).to(dev)

@@ -47,6 +47,9 @@ void set_dispatch(const char* kernel, const char* fetch = nullptr);
 void set_dispatch_reduce(const char* reduce);
 
 int sm_count();   // cached multiprocessor count of the current device
+// per-device caches (function attributes such as a dynamic shared memory opt-in are set per device) are indexed by the
+// device ordinal
+constexpr int kMaxDevices = 64;
 int tune_get(const char* key, int dflt, int lo, int hi);   // runtime knob set through cb200_tune()
 
 // ---- PTX wrappers: mbarrier + bulk async copies (TMA, 1-D form; SASS: UBLKCP / SYNCS) ---------------------------

@@ -328,8 +328,10 @@ __global__ void __launch_bounds__(kC51Warps * 32) c51_head_kernel(C51Params p) {
             const double bj = __ddiv_rn(__dsub_rn(tz, z0), dz);
             const double u = ceil(bj), l = floor(bj);
             const double pj = (double)s_p[j];
-            s_m[(int)l] = __dadd_rn(s_m[(int)l], __dmul_rn(pj, __dsub_rn(u, bj)));
-            s_m[(int)u] = __dadd_rn(s_m[(int)u], __dmul_rn(pj, __dsub_rn(bj, l)));
+            // (z[N-1] - z[0]) / (z[1] - z[0]) of a linspace support can round above N - 1: a share that lands on bin N
+            // is dropped (s_m[N] is the next warp's row)
+            if ((int)l < N) s_m[(int)l] = __dadd_rn(s_m[(int)l], __dmul_rn(pj, __dsub_rn(u, bj)));
+            if ((int)u < N) s_m[(int)u] = __dadd_rn(s_m[(int)u], __dmul_rn(pj, __dsub_rn(bj, l)));
         }
     }
     __syncwarp();
@@ -579,6 +581,18 @@ int cb200_c51_head(const float* next, const float* online, const float* select, 
     p.labels = labels; p.dlogits = dlogits; p.loss_rows = loss_rows; p.td_err = td_err; p.q_online = q_online;
     p.target_actions = target_actions;
     const size_t smem = (size_t)kC51Warps * n_atoms * (sizeof(double) + 2 * sizeof(float));
+    // above 768 atoms the kernel needs more than the 48 KB default (64 KB at 1024): opted into once per device
+    if (smem > 48 * 1024) {
+        static bool attr_set[kMaxDevices] = {};
+        int dev = 0;
+        CB200_CUDA(cudaGetDevice(&dev));
+        CB200_CHECK_ARG(dev < kMaxDevices, "device ordinal out of range");
+        if (!attr_set[dev]) {
+            CB200_CUDA(cudaFuncSetAttribute(c51_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            kC51Warps * 1024 * (int)(sizeof(double) + 2 * sizeof(float))));
+            attr_set[dev] = true;
+        }
+    }
     CB200_LAUNCH(c51_head_kernel, (unsigned)((batch + kC51Warps - 1) / kC51Warps), kC51Warps * 32, smem,
                  as_stream(stream), p);
     CB200_CHECK_LAUNCH();

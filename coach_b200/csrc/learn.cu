@@ -878,17 +878,21 @@ int cb200_ensemble_head_fused(const cb200_ensemble_head_desc* d, void* stream) {
     const int nparts = (int)grid * kHeadWarps;
     cudaStream_t st = as_stream(stream);
     // <= 32 KB of staged head kernels + 32 KB of dz rows: above the 48 KB default, opted into once per instantiation
+    // and device (the attribute is per device: one replay shard per GPU launches it on each)
     const size_t smem = (size_t)(2 * p.A * p.K + kHeadWarps * kHeadRows * p.K) * sizeof(float);
-    static bool attr_set[2] = {false, false};
+    static bool attr_set[kMaxDevices][2] = {};
+    int dev = 0;
+    CB200_CUDA(cudaGetDevice(&dev));
+    CB200_CHECK_ARG(dev < kMaxDevices, "device ordinal out of range");
     const int ti = p.K == 512 ? 1 : 0;
-    if (!attr_set[ti]) {
+    if (!attr_set[dev][ti]) {
         if (ti)
             CB200_CUDA(cudaFuncSetAttribute(ensemble_head_fused_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             64 * 1024));
         else
             CB200_CUDA(cudaFuncSetAttribute(ensemble_head_fused_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                             64 * 1024));
-        attr_set[ti] = true;
+        attr_set[dev][ti] = true;
     }
     if (p.K == 512) {
         CB200_LAUNCH(ensemble_head_fused_kernel<16>, grid, 32 * kHeadWarps, smem, st, p);

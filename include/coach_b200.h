@@ -412,7 +412,8 @@ typedef struct cb200_dqn_head_desc {
      *   PAL (pal_agent.py:70-106): t0 = (float)y; adv = max Qt(s) - Qt(s)[a]; nadv = max Qt(s') - Qt(s')[a*];
      *     m = adv (PAL) or min(adv, nadv) (persistent: nadv only when strictly smaller); t1 = t0 - (float)alpha m;
      *     t2 = (float)(1 - rho) t1; target = (float)((double)t2 + rho R) -- fp32 steps, as numpy evaluates them.
-     * td_err is |target - Q(s, a)| of the final target for these rules. */
+     * td_err is |target - Q(s, a)| of the final target for these rules.  Under every rule, a row whose action is outside
+     * [0, n_actions) keeps Q(s) as its targets (dL/dQ = 0) and gets td_err = 0. */
     int32_t target_rule;
     const float* h_target_s;    /* PAL: [batch, features] features of s from the TARGET network                            */
     const double* mc_returns;   /* MMC / PAL: [batch] Monte Carlo returns (the replay's n_step_discounted_rewards)         */
@@ -579,7 +580,11 @@ int cb200_td3_smooth_actions(float* actions, const double* noise, int64_t n, dou
  * loss_rows [batch, n_actions] = tf.nn.softmax_cross_entropy_with_logits, total_loss = their sum
  * (general_network.py:360), td_err = loss_rows[b, action[b]] (what update_priorities is handed, :160-163), optional
  * q_online [batch, n_actions] fp64 (distribution_prediction_to_q_values) and target_actions.  next_is_prob != 0: `next`
- * / `select` already hold probabilities (parity tests feed the fixture's network outputs). */
+ * / `select` already hold probabilities (parity tests feed the fixture's network outputs).  n_atoms 2 .. 1024 (above
+ * 768 the kernel opts into more than 48 KB of dynamic shared memory).  The projection never writes outside the sample's
+ * row: when (z[N-1] - z[0]) / (z[1] - z[0]) rounds above N - 1 (np.linspace supports often do) and a target clamps to
+ * z[N-1], the share that would land on bin N is dropped -- the reference raises IndexError on the same sample; every
+ * in-row share is unchanged. */
 int cb200_c51_head(const float* next, const float* online, const float* select, const int64_t* actions,
                    const double* rewards, const uint8_t* game_overs, const double* bootstrap, const double* z,
                    double gamma_n, int32_t batch, int32_t n_actions, int32_t n_atoms, int32_t next_is_prob,
