@@ -82,6 +82,15 @@ class EnsembleHeadDesc(ctypes.Structure):
                 ("dh_plane_stride", c_i64), ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p)]
 
 
+class NafHeadDesc(ctypes.Structure):
+    """struct cb200_naf_head_desc"""
+    _fields_ = [("z_v", c_void_p), ("z_mu", c_void_p), ("l", c_void_p), ("scale", c_void_p), ("actions", c_void_p),
+                ("targets", c_void_p), ("huber", ctypes.c_int32), ("batch", c_i64), ("n_actions", ctypes.c_int32),
+                ("ld_mu", ctypes.c_int32), ("ld_l", ctypes.c_int32), ("ld_actions", ctypes.c_int32),
+                ("mu", c_void_p), ("q", c_void_p), ("loss", c_void_p), ("d_zv", c_void_p), ("d_zmu", c_void_p),
+                ("d_l", c_void_p), ("adv", c_void_p)]
+
+
 # cb200_ensemble_action_values modes
 ENSEMBLE_SELECT, ENSEMBLE_UCB, ENSEMBLE_MEAN, ENSEMBLE_VOTE = 0, 1, 2, 3
 
@@ -165,6 +174,8 @@ PROTOTYPES = {
                                ctypes.c_int32, c_void_p]),
     "cb200_ac_td_targets": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_int32, c_i64, c_double, ctypes.c_int32,
                                     ctypes.c_int32, c_double, c_double, c_void_p, c_void_p]),
+    "cb200_naf_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_clip_by_value": (c_int, [c_void_p, c_i64, c_float, c_void_p]),
     "cb200_min2": (c_int, [c_void_p, c_void_p, c_i64, c_void_p, c_void_p]),
     "cb200_td3_smooth_actions": (c_int, [c_void_p, c_void_p, c_i64, c_double, c_double, c_double, c_void_p]),
     "cb200_c51_head": (c_int, [c_void_p] * 8 + [c_double, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,

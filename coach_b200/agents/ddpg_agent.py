@@ -143,9 +143,21 @@ class _Net(object):
         _lib.check(self.lib.cb200_polyak(self.target.data_ptr(), self.store.theta.data_ptr(), self.store.size,
                                          float(rate), _lib.current_stream()))
 
-    def apply(self, ws):
+    def apply(self, ws, clip=None):
+        """clip: None (no clipping) or (gradients_clipping_method, clip_gradients) with "ClipByValue" or
+        "ClipByGlobalNorm": applied to this worker's gradients after their (unclipped) norm is taken and before the
+        all-reduce (architecture.py:193-194, 237-245)"""
         st, s, p = _lib.current_stream(), self.store, self.params
         _lib.check(self.lib.cb200_sumsq(s.grad.data_ptr(), s.size, self.sumsq.data_ptr(), ws.ptr(), st))
+        if clip is not None:
+            method, c = clip
+            if method == "ClipByValue":
+                _lib.check(self.lib.cb200_clip_by_value(s.grad.data_ptr(), s.size, float(c), st))
+            elif method == "ClipByGlobalNorm":
+                _lib.check(self.lib.cb200_clip_by_global_norm(s.grad.data_ptr(), s.size, self.sumsq.data_ptr(),
+                                                              float(c), st))
+            else:
+                raise NotImplementedError("gradient clipping method %r" % (method,))
         scaler = parallel.allreduce_gradients(s.grad, p.scale_down_gradients_by_number_of_workers_for_sync_training)
         if scaler != 1.0:
             _lib.check(self.lib.cb200_scale(s.grad.data_ptr(), s.size, float(scaler), st))

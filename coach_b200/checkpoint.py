@@ -176,7 +176,7 @@ def _network_items(agent):
         if w.theta_target is not None:
             extra["target"] = w.theta_target
         out.append(("main", w.store, extra, w))
-    for tag in ("actor", "critic", "policy", "q", "v"):                                       # _Net based agents
+    for tag in ("main", "actor", "critic", "policy", "q", "v"):                               # _Net based agents
         net = getattr(agent, tag, None)
         if net is not None and hasattr(net, "store") and hasattr(net, "adam_state"):
             out.append((tag, net.store, {"adam_state": net.adam_state, "target": net.target}, net))

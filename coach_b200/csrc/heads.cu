@@ -480,11 +480,149 @@ __global__ void __launch_bounds__(256) f64_to_f32_kernel(const double* __restric
     if (i < n) out[i] = (float)in[i];
 }
 
+// =====================================================================================================================
+// NAFHead (heads/naf_head.py:45-86), see cb200_naf_head in the header.  One warp per sample; lane c owns action c and
+// column c of L.  The sample's packed l vector is staged in shared memory (coalesced), so that lane c reads its column
+// for w_c = sum_{r >= c} L[r, c] d_r and lane r its row for (L w)_r = sum_{c <= r} L[r, c] w_c; d and w travel by
+// shuffles.  |w|^2 is an xor butterfly, which leaves the same bits in every lane.  The d_l column of each lane is
+// written back into the staging buffer and stored coalesced.
+constexpr int kNafWarps = 8;
+constexpr int kNafMaxL = kMaxActionDim * (kMaxActionDim + 1) / 2;
+
+struct NafParams {
+    const float *z_v, *z_mu, *l, *scale, *actions, *targets;
+    int huber, A, ld_mu, ld_l, ld_u;
+    int64_t B;
+    float *mu, *q, *d_zv, *d_zmu, *d_l, *adv;
+};
+
+// Huber (delta 1) / squared error of e = Q - y and the derivative dl/dQ, as regression_head_kernel (learn.cu) has them
+__device__ __forceinline__ void naf_loss_terms(float e, int huber, float& l, float& g) {
+    if (huber) {
+        const float ae = fabsf(e);
+        const float q = fminf(ae, 1.0f);
+        l = 0.5f * q * q + (ae - q);
+        g = (ae <= 1.0f) ? e : (e > 0.f ? 1.0f : -1.0f);
+    } else {
+        l = e * e;
+        g = 2.0f * e;
+    }
+}
+
+template <bool kTrain>
+__global__ void __launch_bounds__(kNafWarps * 32) naf_head_kernel(const NafParams p) {
+    __shared__ float s_l[kNafWarps][kNafMaxL];
+    const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+    const int64_t b = (int64_t)blockIdx.x * kNafWarps + wib;
+    if (b >= p.B) return;                                              // whole warps only
+    const int A = p.A;
+    const bool own = lane < A;
+    float t = 0.f, mu = 0.f;
+    if (own) {
+        t = tanhf(p.z_mu[b * p.ld_mu + lane]);
+        mu = t * p.scale[lane];
+        p.mu[b * p.ld_mu + lane] = mu;
+    }
+    if (!kTrain) {
+        if (lane == 0 && p.q) p.q[b] = p.z_v[b];                       // u = mu: the advantage is 0
+        return;
+    }
+    const float v = p.z_v[b];
+    float* ls = s_l[wib];
+    const int nl = A * (A + 1) / 2;
+    for (int k = lane; k < nl; k += 32) ls[k] = p.l[b * p.ld_l + k];
+    __syncwarp();
+    const float d = own ? p.actions[b * p.ld_u + lane] - mu : 0.f;
+    const int ic = lane * A - lane * (lane - 1) / 2;                   // start of column `lane`
+    const float diag = own ? expf(ls[ic]) : 0.f;
+    // w_c = sum_{r >= c} L[r, c] d_r
+    float w = 0.f;
+    for (int r = 0; r < A; ++r) {
+        const float dr = __shfl_sync(0xffffffffu, d, r);
+        if (own && r >= lane) w = fmaf(r == lane ? diag : ls[ic + r - lane], dr, w);
+    }
+    float ww = w * w;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ww += __shfl_xor_sync(0xffffffffu, ww, o);
+    const float adv = -0.5f * ww;
+    const float qv = v + adv;
+    float lterm, g;
+    naf_loss_terms(qv - p.targets[b], p.huber, lterm, g);
+    const float dq = (1.0f / (float)p.B) * g;
+    // (L w)_r = sum_{c <= r} L[r, c] w_c = dA/dmu_r
+    float lw = 0.f;
+    for (int c = 0; c < A; ++c) {
+        const float wc = __shfl_sync(0xffffffffu, w, c);
+        const int icc = c * A - c * (c - 1) / 2;
+        if (own && c <= lane) lw = fmaf(c == lane ? diag : ls[icc + lane - c], wc, lw);
+    }
+    if (own) p.d_zmu[b * p.ld_mu + lane] = dq * lw * p.scale[lane] * (1.0f - t * t);
+    if (lane == 0) {
+        p.q[b] = qv;
+        p.d_zv[b] = dq;
+        if (p.adv) p.adv[b] = adv;
+    }
+    __syncwarp();                                                      // every read of the staged l is done
+    // dA/dL[r, c] = -d_r w_c; the diagonal entries are exp(l): times L[c, c]
+    for (int r = 0; r < A; ++r) {
+        const float dr = __shfl_sync(0xffffffffu, d, r);
+        if (own && r >= lane) {
+            const float gl = dq * (-dr * w);
+            ls[ic + r - lane] = r == lane ? gl * diag : gl;
+        }
+    }
+    __syncwarp();
+    for (int k = lane; k < nl; k += 32) p.d_l[b * p.ld_l + k] = ls[k];
+}
+
+// loss = mean_b l(q_b - y_b) in a fixed order (the per-thread strided sums and the tree of regression_head_kernel)
+__global__ void __launch_bounds__(256) naf_loss_kernel(const float* __restrict__ q, const float* __restrict__ targets,
+                                                       int64_t B, int huber, float* __restrict__ loss) {
+    __shared__ float red[256];
+    float local = 0.f;
+    for (int64_t b = threadIdx.x; b < B; b += blockDim.x) {
+        float l, g;
+        naf_loss_terms(q[b] - targets[b], huber, l, g);
+        local += l;
+    }
+    const float s = block_sum(local, red);
+    if (threadIdx.x == 0) *loss = s * (1.0f / (float)B);
+}
+
 }  // namespace cb200
 
 using namespace cb200;
 
 extern "C" {
+
+int cb200_naf_head(const cb200_naf_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->n_actions >= 1 && d->n_actions <= kMaxActionDim, "1 <= n_actions <= 32");
+    CB200_CHECK_ARG(d->batch > 0 && d->batch <= (int64_t)0x7fffffff * kNafWarps, "bad batch");
+    CB200_CHECK_ARG(d->z_mu && d->scale && d->mu, "null pointer (z_mu, scale, mu)");
+    CB200_CHECK_ARG(!d->actions == !d->targets, "actions and targets are both given (training) or both NULL (acting)");
+    const bool train = d->actions != nullptr;
+    CB200_CHECK_ARG(!(train || d->q) || d->z_v, "q needs z_v");
+    CB200_CHECK_ARG(!train || (d->l && d->q && d->loss && d->d_zv && d->d_zmu && d->d_l),
+                    "training needs l, q, loss, d_zv, d_zmu and d_l");
+    const int A = d->n_actions;
+    CB200_CHECK_ARG(d->ld_mu >= A && (!train || (d->ld_l >= A * (A + 1) / 2 && d->ld_actions >= A)),
+                    "leading dimensions below the row widths");
+    NafParams p;
+    p.z_v = d->z_v; p.z_mu = d->z_mu; p.l = d->l; p.scale = d->scale; p.actions = d->actions; p.targets = d->targets;
+    p.huber = d->huber; p.A = A; p.ld_mu = d->ld_mu; p.ld_l = d->ld_l; p.ld_u = d->ld_actions; p.B = d->batch;
+    p.mu = d->mu; p.q = d->q; p.d_zv = d->d_zv; p.d_zmu = d->d_zmu; p.d_l = d->d_l; p.adv = d->adv;
+    const unsigned grid = (unsigned)((d->batch + kNafWarps - 1) / kNafWarps);
+    cudaStream_t st = as_stream(stream);
+    if (train) {
+        CB200_LAUNCH(naf_head_kernel<true>, grid, kNafWarps * 32, 0, st, p);
+        CB200_LAUNCH(naf_loss_kernel, 1, 256, 0, st, d->q, d->targets, d->batch, d->huber, d->loss);
+    } else {
+        CB200_LAUNCH(naf_head_kernel<false>, grid, kNafWarps * 32, 0, st, p);
+    }
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
 
 int cb200_ppo_continuous_head(const float* mu, const float* logstd, const float* actions, const float* old_mu,
                               const float* old_logstd, const float* advantages, int64_t batch, int32_t action_dim,

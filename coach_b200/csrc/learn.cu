@@ -695,6 +695,13 @@ __global__ void __launch_bounds__(256) clip_kernel(float* __restrict__ g, int64_
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         g[i] *= scale;
 }
+// tf.clip_by_value: the comparisons are false for NaN, which passes through unchanged
+__global__ void __launch_bounds__(256) clip_by_value_kernel(float* __restrict__ g, int64_t n, float clip) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const float x = g[i];
+        g[i] = x < -clip ? -clip : (x > clip ? clip : x);
+    }
+}
 __global__ void __launch_bounds__(256) scale_kernel(float* __restrict__ g, int64_t n, float s) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         g[i] *= s;
@@ -949,6 +956,13 @@ int cb200_sumsq(const float* x, int64_t n, float* out, float* workspace, void* s
 int cb200_clip_by_global_norm(float* g, int64_t n, const float* sumsq, float clip, void* stream) {
     CB200_CHECK_ARG(g && sumsq && n > 0 && clip > 0, "bad arguments");
     CB200_LAUNCH(clip_kernel, flat_grid(n), 256, 0, as_stream(stream), g, n, sumsq, clip);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_clip_by_value(float* g, int64_t n, float clip, void* stream) {
+    CB200_CHECK_ARG(g && n > 0 && clip > 0, "bad arguments");
+    CB200_LAUNCH(clip_by_value_kernel, flat_grid(n), 256, 0, as_stream(stream), g, n, clip);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

@@ -561,6 +561,47 @@ int cb200_ac_td_targets(const double* rewards, const uint8_t* game_overs, const 
                         int64_t batch, double discount, int32_t use_non_zero_discount_for_terminal_states,
                         int32_t use_clip, double clip_lo, double clip_hi, float* targets_out, void* stream);
 
+/* NAFHead (heads/naf_head.py:45-86), the per-sample nonlinear part: the three head projections come from ordinary Dense
+ * layers (V: 1 output, mu: n_actions pre-tanh outputs, l: n_actions (n_actions + 1) / 2 outputs).  Per sample b:
+ *   mu = tanh(z_mu) * scale                                    (scale: max_abs_range rounded to fp32)
+ *   L  = lower triangle of l packed column by column: column c holds rows c .. A-1, starting at
+ *        i_c = c A - c (c - 1) / 2, with L[c, c] = exp(l[i_c])
+ *   d  = u - mu,  w = L^T d,  adv = -0.5 * d^T L L^T d = -0.5 * |w|^2,  Q = V + adv
+ *   loss = mean_b l(Q_b - y_b), l = squared error or Huber (delta 1) (head.py:165-177; no importance weights)
+ * and the gradients of the loss straight into the three layers' output gradients:
+ *   d_zv = dL/dQ,  d_zmu = dL/dQ * (L w) * scale * (1 - tanh^2),  d_l[L[r, c]] = dL/dQ * (-d_r w_c), times L[c, c] on
+ *   the diagonal.
+ * The kernel evaluates w first (not P = L L^T as the TensorFlow graph does); its accuracy is stated against fp64
+ * (tests/test_naf_gpu.py).  One warp per sample, n_actions <= 32.  The loss is reduced in a fixed order by a second
+ * launch: the same bits on every call.
+ * Acting mode (actions == NULL and targets == NULL): only mu and -- when given -- q = V are written; l, ld_l and
+ * ld_actions are not read, and z_v only when q is given.
+ * mu / z_mu / d_zmu use the row stride ld_mu, l / d_l ld_l, actions ld_actions; z_v, q, targets, d_zv, adv are [batch]. */
+typedef struct cb200_naf_head_desc {
+    const float* z_v;           /* [batch] V projection (acting: only read when q is given)                          */
+    const float* z_mu;          /* [batch, ld_mu] mu projection before the tanh                                      */
+    const float* l;             /* [batch, ld_l] l_vector projection (training only)                                 */
+    const float* scale;         /* [n_actions] output scale of mu                                                    */
+    const float* actions;       /* [batch, ld_actions] the head input u (the batch actions); NULL: acting mode       */
+    const float* targets;       /* [batch] TD targets; NULL: acting mode                                             */
+    int32_t huber;              /* replace_mse_with_huber_loss                                                       */
+    int64_t batch;
+    int32_t n_actions;          /* 1 .. 32                                                                           */
+    int32_t ld_mu, ld_l, ld_actions;
+    float* mu;                  /* [batch, ld_mu] scaled mu (always written)                                         */
+    float* q;                   /* [batch] Q (training: required; acting: optional, = V)                             */
+    float* loss;                /* [1] training: required                                                            */
+    float* d_zv;                /* [batch] training: required                                                        */
+    float* d_zmu;               /* [batch, ld_mu] training: required                                                 */
+    float* d_l;                 /* [batch, ld_l] training: required                                                  */
+    float* adv;                 /* [batch] training: optional                                                        */
+} cb200_naf_head_desc;
+int cb200_naf_head(const cb200_naf_head_desc* desc, void* stream);
+
+/* tf.clip_by_value(g, -clip, clip) in place (architecture.py:241-245, GradientClippingMethod.ClipByValue); NaN passes
+ * through, +-inf clips.  clip > 0. */
+int cb200_clip_by_value(float* g, int64_t n, float clip, void* stream);
+
 /* out = min(a, b) element-wise (clipped double-Q: td3_v_head.py:61, sac_q_head.py:84-86) */
 int cb200_min2(const float* a, const float* b, int64_t n, float* out, void* stream);
 
