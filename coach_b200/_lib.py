@@ -91,6 +91,14 @@ class NafHeadDesc(ctypes.Structure):
                 ("d_l", c_void_p), ("adv", c_void_p)]
 
 
+class QrHeadDesc(ctypes.Structure):
+    """struct cb200_qr_head_desc"""
+    _fields_ = [("next", c_void_p), ("online", c_void_p), ("actions", c_void_p), ("rewards", c_void_p),
+                ("game_overs", c_void_p), ("discount", c_double), ("kappa", c_float), ("batch", ctypes.c_int32),
+                ("n_actions", ctypes.c_int32), ("n_atoms", ctypes.c_int32), ("dq", c_void_p), ("loss", c_void_p),
+                ("targets", c_void_p), ("taus", c_void_p), ("target_actions", c_void_p), ("workspace", c_void_p)]
+
+
 # cb200_ensemble_action_values modes
 ENSEMBLE_SELECT, ENSEMBLE_UCB, ENSEMBLE_MEAN, ENSEMBLE_VOTE = 0, 1, 2, 3
 
@@ -181,6 +189,8 @@ PROTOTYPES = {
     "cb200_c51_head": (c_int, [c_void_p] * 8 + [c_double, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32,
                                ctypes.c_int32] + [c_void_p] * 8),
     "cb200_c51_q_values": (c_int, [c_void_p, c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p]),
+    "cb200_qr_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_qr_q_values": (c_int, [c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p]),
     "cb200_gae_scan": (c_int, [c_void_p, c_void_p, c_void_p, c_i64, c_double, c_double, c_void_p, c_void_p, c_void_p,
                                c_void_p]),
     "cb200_standardize": (c_int, [c_void_p, c_i64, c_void_p, c_void_p, c_void_p]),

@@ -589,6 +589,143 @@ __global__ void __launch_bounds__(256) naf_loss_kernel(const float* __restrict__
     if (threadIdx.x == 0) *loss = s * (1.0f / (float)B);
 }
 
+// =====================================================================================================================
+// QuantileRegressionQHead + the TD targets of QuantileRegressionDQNAgent (agents/qr_dqn_agent.py:97-137,
+// heads/quantile_regression_q_head.py:33-71), see cb200_qr_head in the header.  One CTA per sample:
+//   Q'[a]   = sum_j (double)next[a, j] * (1.0 / N)        (qr_row_q; one warp per action)
+//   a*      = first argmax of Q'
+//   T_j     = (float)(r + ((1.0 - done) * gamma) * (double)next[a*, j])              (fp64, _rn: the numpy expression)
+//   sigma   = argsort of the taken row, ties by index;  tau_i = (float)tau_hat[sigma(i)]   (the reference's permutation)
+//   thread i: the pair terms (i, j) for j = 0 .. N-1 in order, in fp32 without contraction; the loss sums in fp32, the
+//             gradient's terms (of both signs) in fp64
+// The per-sample loss goes to the workspace; qr_loss_kernel sums it in a fixed order: the same bits on every call.
+// =====================================================================================================================
+constexpr int kQrThreads = 256;
+constexpr int kQrMaxAtoms = 1024;
+constexpr int kQrMaxActions = 256;
+
+// the head's q_values for one row of N quantiles (np.dot with ones(N) / N in fp64): lanes stride j, then an xor
+// butterfly, which leaves the same bits in every lane
+__device__ __forceinline__ double qr_row_q(const float* __restrict__ row, int N, int lane) {
+    const double p = __ddiv_rn(1.0, (double)N);
+    double acc = 0.0;
+    for (int j = lane; j < N; j += 32) acc = __dadd_rn(acc, __dmul_rn((double)row[j], p));
+    return warp_sum(acc);
+}
+
+struct QrParams {
+    const float* next; const float* online; const int64_t* actions; const double* rewards; const uint8_t* game_overs;
+    double discount;
+    float kappa;
+    int B, A, N;
+    float* dq; float* targets; float* taus; int64_t* target_actions; float* partial;
+};
+
+__global__ void __launch_bounds__(kQrThreads) qr_head_kernel(const QrParams p) {
+    __shared__ float s_theta[kQrMaxAtoms], s_t[kQrMaxAtoms], s_tau[kQrMaxAtoms], s_g[kQrMaxAtoms];
+    __shared__ int s_sigma[kQrMaxAtoms];
+    __shared__ double s_q[kQrMaxActions];
+    __shared__ float red[kQrThreads];
+    __shared__ int s_best;
+    const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int A = p.A, N = p.N;
+    const int64_t row = (int64_t)b * A * N;
+    // ---- Q' and the target action ------------------------------------------------------------------------------------
+    for (int a = warp; a < A; a += kQrThreads / 32) {
+        const double q = qr_row_q(p.next + row + (int64_t)a * N, N, lane);
+        if (lane == 0) s_q[a] = q;
+    }
+    const int64_t act64 = p.actions[b];
+    const bool valid = act64 >= 0 && act64 < A;
+    const int act = valid ? (int)act64 : 0;
+    for (int i = tid; i < N; i += kQrThreads) {
+        s_theta[i] = p.online[row + (int64_t)act * N + i];
+        s_sigma[i] = i;                      // every slot holds an index even if NaNs make the ranks collide
+    }
+    __syncthreads();
+    if (tid == 0) {
+        int best = 0;
+        for (int a = 1; a < A; ++a)
+            if (s_q[a] > s_q[best]) best = a;                                    // np.argmax: first maximum
+        s_best = best;
+        if (p.target_actions) p.target_actions[b] = best;
+    }
+    // ---- ranks of the taken row (index tie-break = argsort kind='stable') --------------------------------------------
+    for (int i = tid; i < N; i += kQrThreads) {
+        const float v = s_theta[i];
+        int r = 0;
+        for (int k = 0; k < N; ++k) {
+            const float u = s_theta[k];
+            r += (u < v || (u == v && k < i)) ? 1 : 0;
+        }
+        s_sigma[r] = i;                                                          // sigma = argsort: sigma(rank(i)) = i
+    }
+    __syncthreads();
+    // ---- TD targets and the permuted midpoints -----------------------------------------------------------------------
+    const int best = s_best;
+    const double coef = __dmul_rn(__dsub_rn(1.0, p.game_overs[b] ? 1.0 : 0.0), p.discount);
+    const double r = p.rewards[b];
+    for (int j = tid; j < N; j += kQrThreads) {
+        const float t = __double2float_rn(__dadd_rn(r, __dmul_rn(coef, (double)p.next[row + (int64_t)best * N + j])));
+        s_t[j] = t;
+        if (p.targets) p.targets[(int64_t)b * N + j] = t;
+        // tau_hat_k = 0.5 * (c[k + 1] + c[k]), c = arange(N + 1) / N in fp64
+        const int k = s_sigma[j];
+        const double mid = __dmul_rn(0.5, __dadd_rn(__ddiv_rn((double)(k + 1), (double)N),
+                                                    __ddiv_rn((double)k, (double)N)));
+        s_tau[j] = __double2float_rn(mid);
+        if (p.taus && valid) p.taus[(int64_t)b * N + j] = s_tau[j];
+    }
+    __syncthreads();
+    // ---- pair terms: thread i owns theta_i and sums over j in order ---------------------------------------------------
+    const float kappa = p.kappa;
+    const double inv_n = __ddiv_rn(1.0, (double)N);
+    float loss = 0.f;
+    for (int i = tid; i < N; i += kQrThreads) {
+        const float th = s_theta[i], tau = s_tau[i];
+        float li = 0.f;
+        double gi = 0.0;                       // the gradient's j-sum cancels: accumulated in fp64, rounded once
+        for (int j = 0; j < N; ++j) {
+            const float e = __fsub_rn(s_t[j], th);
+            const float ae = fabsf(e);
+            const float q = fminf(ae, kappa);
+            const float h = __fadd_rn(__fmul_rn(kappa, __fsub_rn(ae, q)), __fmul_rn(0.5f, __fmul_rn(q, q)));
+            const float w = fabsf(__fsub_rn(tau, e < 0.f ? 1.0f : 0.0f));
+            li = __fadd_rn(li, __fmul_rn(w, h));
+            gi = __dadd_rn(gi, (double)__fmul_rn(w, fminf(fmaxf(e, -kappa), kappa)));
+        }
+        loss = __fadd_rn(loss, li);
+        s_g[i] = valid ? __double2float_rn(__dmul_rn(-gi, inv_n)) : 0.f;
+    }
+    const float total = block_sum(valid ? loss : 0.f, red);                     // (its barriers also publish s_g)
+    if (tid == 0) p.partial[b] = total;
+    // ---- d loss / d quantiles: the taken row, 0 on every other action --------------------------------------------------
+    for (int k = tid; k < A * N; k += kQrThreads) {
+        const int a = k / N;
+        p.dq[row + k] = (valid && a == act) ? s_g[k - a * N] : 0.f;
+    }
+}
+
+// loss = (sum_b partial[b]) / N: one block, the strided per-thread sums and the tree of block_sum
+__global__ void __launch_bounds__(256) qr_loss_kernel(const float* __restrict__ partial, int B, int N,
+                                                      float* __restrict__ loss) {
+    __shared__ float red[256];
+    float v = 0.f;
+    for (int b = threadIdx.x; b < B; b += 256) v = __fadd_rn(v, partial[b]);
+    const float s = block_sum(v, red);
+    if (threadIdx.x == 0) *loss = __fdiv_rn(s, (float)N);
+}
+
+// q_values of the QuantileRegressionQHead for acting, one warp per (b, a) row
+__global__ void __launch_bounds__(128) qr_q_values_kernel(const float* __restrict__ quantiles, int64_t rows, int N,
+                                                          double* __restrict__ q) {
+    const int64_t r = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (r >= rows) return;
+    const double v = qr_row_q(quantiles + r * N, N, lane);
+    if (lane == 0) q[r] = v;
+}
+
 }  // namespace cb200
 
 using namespace cb200;
@@ -620,6 +757,37 @@ int cb200_naf_head(const cb200_naf_head_desc* d, void* stream) {
     } else {
         CB200_LAUNCH(naf_head_kernel<false>, grid, kNafWarps * 32, 0, st, p);
     }
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_qr_head(const cb200_qr_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->n_atoms >= 1 && d->n_atoms <= kQrMaxAtoms, "1 <= n_atoms <= 1024");
+    CB200_CHECK_ARG(d->n_actions >= 1 && d->n_actions <= kQrMaxActions, "1 <= n_actions <= 256");
+    CB200_CHECK_ARG(d->batch >= 1, "batch >= 1");
+    CB200_CHECK_ARG(d->kappa >= 0.f && d->kappa <= INFINITY, "huber_loss_interval >= 0");
+    CB200_CHECK_ARG(d->next && d->online && d->actions && d->rewards && d->game_overs,
+                    "null input (next, online, actions, rewards, game_overs)");
+    CB200_CHECK_ARG(d->dq && d->loss && d->workspace, "null output (dq, loss, workspace)");
+    QrParams p;
+    p.next = d->next; p.online = d->online; p.actions = d->actions; p.rewards = d->rewards;
+    p.game_overs = d->game_overs; p.discount = d->discount; p.kappa = d->kappa;
+    p.B = d->batch; p.A = d->n_actions; p.N = d->n_atoms;
+    p.dq = d->dq; p.targets = d->targets; p.taus = d->taus; p.target_actions = d->target_actions;
+    p.partial = d->workspace;
+    cudaStream_t st = as_stream(stream);
+    CB200_LAUNCH(qr_head_kernel, (unsigned)d->batch, kQrThreads, 0, st, p);
+    CB200_CHECK_LAUNCH();
+    CB200_LAUNCH(qr_loss_kernel, 1, 256, 0, st, d->workspace, d->batch, d->n_atoms, d->loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_qr_q_values(const float* quantiles, int64_t rows, int32_t n_atoms, double* q_out, void* stream) {
+    CB200_CHECK_ARG(quantiles && q_out && rows > 0 && n_atoms >= 1 && n_atoms <= kQrMaxAtoms, "bad arguments");
+    CB200_LAUNCH(qr_q_values_kernel, (unsigned)((rows + 3) / 4), 128, 0, as_stream(stream), quantiles, rows, n_atoms,
+                 q_out);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

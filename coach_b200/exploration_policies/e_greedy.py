@@ -10,11 +10,26 @@ in one [E, A] read-back (a few hundred bytes); the arithmetic on them is the ref
 """
 import numpy as np
 
-from coach_b200.schedules import Schedule
+from coach_b200.schedules import LinearSchedule, Schedule
 
 
 class RunPhase(object):
     HEATUP, TRAIN, TEST = "Heatup", "Training", "Testing"
+
+
+class EGreedyParameters(object):
+    """exploration_policies/e_greedy.py:29-41, discrete action spaces (the continuous fall-back is not carried)"""
+
+    def __init__(self):
+        self.epsilon_schedule = LinearSchedule(0.5, 0.01, 50000)
+        self.evaluation_epsilon = 0.05
+
+    @property
+    def path(self):
+        return 'coach_b200.exploration_policies.e_greedy:BatchedEGreedy'
+
+    def make(self, num_actions, num_envs):
+        return BatchedEGreedy(num_actions, num_envs, self.epsilon_schedule, self.evaluation_epsilon)
 
 
 class BatchedEGreedy(object):

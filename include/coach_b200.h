@@ -636,6 +636,51 @@ int cb200_c51_head(const float* next, const float* online, const float* select, 
  * for rows = batch * n_actions rows of n_atoms logits; z = the fp32-rounded support cast back to fp64 (:36-37) */
 int cb200_c51_q_values(const float* logits, const double* z, int64_t rows, int32_t n_atoms, double* q_out, void* stream);
 
+/* QuantileRegressionQHead + the TD targets of QuantileRegressionDQNAgent (agents/qr_dqn_agent.py:97-137,
+ * heads/quantile_regression_q_head.py:33-71).  Inputs are the [batch, n_actions, n_atoms] quantiles of target(s') and
+ * online(s) (action-major, atom-inner).  Per sample b, with N = n_atoms:
+ *   Q'[a]    = sum_j (double)next[a, j] * (1.0 / N) in fp64 (the head's q_values, np.dot with ones(N) / N);
+ *              a* = the first argmax of Q'.  numpy's summation order is unspecified: Q' equals the reference's up to
+ *              fp64 rounding, so only a near tie of two actions can choose differently.
+ *   T_j      = (float)(r + ((1.0 - game_over) * discount) * (double)next[a*, j]), each operation an fp64 _rn operation
+ *              in numpy's order: bit-exact with the reference's TD_targets as fed.
+ *   sigma    = argsort of the taken row online[action, :], ties broken by index (kind='stable'); the reference assigns
+ *              tau_i = tau_hat[sigma(i)] (NOT the rank tau_hat[sigma^-1(i)]), tau_hat_k = 0.5 * ((k + 1) / N + k / N)
+ *              in fp64, fed as fp32 -- kept.
+ *   pair (i, j), fp32, no contraction: e = T_j - theta_i, a = |e|, q = min(a, kappa), h = kappa (a - q) + 0.5 q^2,
+ *              l = |tau_i - [e < 0]| h
+ *   loss     = (sum over b, i, j of l) / N: summed over the batch, no importance weights.
+ *   dq       = d loss / d online: -(1/N) sum_j |tau_i - [e < 0]| clamp(e, -kappa, kappa) on the taken row
+ *              (tf.minimum sends its gradient to the first argument on ties), exactly 0 on every other row.  The
+ *              products are fp32; their j-sum, which cancels, is accumulated in fp64 and rounded once.
+ * kappa = 0 (the reference's "strict quantile loss") makes h, the loss and dq identically 0: the reference's
+ * arithmetic, kept.  Each theta_i's j-sum runs in one thread in j order; the per-sample sums go to workspace and a
+ * second launch reduces them in a fixed order: the same bits on every call (eager or graph replay).  An action outside
+ * [0, n_actions) contributes 0 to the loss and dq, and its taus row is not written.  NaN quantiles give an unspecified
+ * (in-range) order.  Limits: 1 <= n_atoms <= 1024, 1 <= n_actions <= 256, batch >= 1, kappa >= 0. */
+typedef struct cb200_qr_head_desc {
+    const float* next;          /* [batch, n_actions * n_atoms] target network on s'                                 */
+    const float* online;        /* [batch, n_actions * n_atoms] online (training) network on s                        */
+    const int64_t* actions;     /* [batch] taken actions                                                              */
+    const double* rewards;      /* [batch]                                                                            */
+    const uint8_t* game_overs;  /* [batch]                                                                            */
+    double discount;
+    float kappa;                /* huber_loss_interval                                                                */
+    int32_t batch, n_actions, n_atoms;
+    float* dq;                  /* [batch, n_actions * n_atoms] d loss / d online (the trunk's output gradient)       */
+    float* loss;                /* [1] total loss                                                                     */
+    float* targets;             /* [batch, n_atoms] optional: T as fed to the train op                                */
+    float* taus;                /* [batch, n_atoms] optional: the quantile midpoints as fed (output_0_1)              */
+    int64_t* target_actions;    /* [batch] optional: a*                                                               */
+    float* workspace;           /* [batch] per-sample loss sums                                                       */
+} cb200_qr_head_desc;
+int cb200_qr_head(const cb200_qr_head_desc* desc, void* stream);
+
+/* q_values output of the QuantileRegressionQHead (quantile_regression_q_head.py:65, qr_dqn_agent.py:72-73):
+ * q[r] = sum_j (double)quantiles[r, j] * (1.0 / n_atoms) for `rows` rows of n_atoms, the arithmetic of Q' in
+ * cb200_qr_head.  1 <= n_atoms <= 1024. */
+int cb200_qr_q_values(const float* quantiles, int64_t rows, int32_t n_atoms, double* q_out, void* stream);
+
 /* SACPolicyHead (heads/sac_head.py:60-97).  head_out [batch, 2*action_dim] = [mu | raw log-sigma]; log-sigma is clipped
  * to [-20, 2]; u = mu + exp(log_sigma) * eps; a = tanh(u); logp = MVN-diag log-prob of u minus the tanh squash
  * correction sum_j log(1 - a_j^2 + 1e-6).  Any output may be NULL. */
