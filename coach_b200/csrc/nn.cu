@@ -681,6 +681,9 @@ int cb200_permute_f32(const float* src, const int32_t* table, int64_t n, float* 
 int cb200_transpose(const float* src, int64_t rows, int64_t cols, float* dst, void* dst_planes, int64_t plane_stride,
                     void* stream) {
     CB200_CHECK_ARG(src && dst && rows > 0 && cols > 0, "bad arguments");
+    // the planes of dst [cols, rows] have rows plane columns: whole 8-column cores, planes on core boundaries
+    CB200_CHECK_ARG(!dst_planes || (rows % 8 == 0 && plane_stride % 8 == 0 && plane_stride >= rows * ((cols + 7) / 8 * 8)),
+                    "planes: rows % 8 == 0, plane_stride % 8 == 0 and >= rows * cols rounded up to 8 rows");
     dim3 grid((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32));
     gemm::transpose_kernel<<<grid, dim3(32, 8), 0, as_stream(stream)>>>(src, rows, cols, dst,
                                                                         static_cast<uint16_t*>(dst_planes), plane_stride);

@@ -343,7 +343,10 @@ int cb200_permute_f32(const float* src, const int32_t* table, int64_t n, float* 
                       int64_t plane_stride, int32_t plane_cols, void* stream);
                       /* dst_planes optional (NULL): also write dst, seen as [n / plane_cols, plane_cols], as planes */
 
-/* dst[c, r] = src[r, c]  (fp32; pre-transposition of weight matrices for the data-gradient GEMMs) */
+/* dst[c, r] = src[r, c]  (fp32; pre-transposition of weight matrices for the data-gradient GEMMs).
+ * dst_planes optional (NULL): also write dst [cols, rows] as core-tiled planes `plane_stride` apart; needs rows % 8 == 0
+ * (whole column cores), plane_stride % 8 == 0 and plane_stride >= rows * cols rounded up to a multiple of 8 rows.  When
+ * cols % 8 != 0 the rows of the last row group past cols are not written. */
 int cb200_transpose(const float* src, int64_t rows, int64_t cols, float* dst, void* dst_planes, int64_t plane_stride,
                     void* stream);
 
@@ -498,7 +501,10 @@ int cb200_dueling_combine_bwd(const float* dq, int64_t batch, int64_t n_actions,
  * sqrt(sum_t sum(t^2)) (architecture.py:194).  workspace >= 1024 floats. */
 int cb200_sumsq(const float* x, int64_t n, float* out, float* workspace, void* stream);
 
-/* tf.clip_by_global_norm (architecture.py:239-240): g *= clip / max(sqrt(*sumsq), clip)  -- in place. */
+/* tf.clip_by_global_norm (architecture.py:239-240): g *= clip / max(sqrt(*sumsq), clip)  -- in place, fp32 (sqrtf and
+ * the division correctly rounded; finite g is untouched bit for bit while sqrt(*sumsq) <= clip).  A non-finite norm: *sumsq =
+ * +inf scales by 0 (finite gradients become +-0), *sumsq = NaN scales by 1 (fmaxf drops the NaN: g passes unclipped,
+ * and the NaN that made the norm NaN is still in g). */
 int cb200_clip_by_global_norm(float* g, int64_t n, const float* sumsq, float clip, void* stream);
 
 /* g *= s (apply_gradients `scaler`, architecture.py:485-493: 1/num_workers for sync training) */
