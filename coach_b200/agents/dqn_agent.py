@@ -210,7 +210,8 @@ class DQNAgent(object):
         if (self.net_def.is_image and B >= 128 and B % 32 == 0 and _lib.tune_default("gemm_tiled", 1) and
                 _lib.tune_default("conv_s2d", 1) and _lib.tune_default("fused_input", 1) and
                 first.KH % first.S == 0 and first.H % first.S == 0 and first.W % first.S == 0 and
-                (first.S * first.C) % 8 == 0 and tl.channels_ok(first.S * first.S * first.C)):
+                (first.S * first.C) % 8 == 0 and tl.channels_ok(first.S * first.S * first.C) and
+                tl.width_ok(first.N)):
             H, W, C, S = first.H, first.W, first.C, first.S
             mk = lambda: tl.PlaneBuf((H // S) * (W // S) * B, S * S * C, dev, npix=(H // S) * (W // S), nplanes=1)  # noqa
             self.s2d = {"columns": {"state:observation": mk(), "next_state:observation": mk()},

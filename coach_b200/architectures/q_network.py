@@ -24,8 +24,11 @@ class QNetworkDef(object):
     """Parameter layout + layer chain; instances bind it to buffers (see QNetworkInstance)."""
 
     def __init__(self, device, observation_shape, num_actions, dueling=False, embedder="auto", middleware_units=512,
-                 head_copies=1, head_grad_rescale=1.0):
-        """middleware_units: width of one FC middleware layer, a tuple of widths, or None / () for MiddlewareScheme.Empty.
+                 head_copies=1, head_grad_rescale=1.0, embedder_scheme=None):
+        """embedder_scheme: the input embedder's layers (InputEmbedderParameters.scheme as a list): for images a list of
+        base_parameters.Conv2d specs, for vectors a list of base_parameters.Dense specs; None is the Medium embedder
+        above (image_embedder.py:62-67 / vector_embedder.py:58-61).
+        middleware_units: width of one FC middleware layer, a tuple of widths, or None / () for MiddlewareScheme.Empty.
         head_copies > 1 (Bootstrapped DQN, bootstrapped_dqn_agent.py:26-30): ``head_copies`` QHeads of ``num_actions``
         outputs on the same features, as ONE Dense(head_copies * num_actions) whose column block [k A, (k + 1) A) is
         head k; each block is Glorot-initialised with the fans of its own [F, A] layer, and there is one
@@ -48,15 +51,19 @@ class QNetworkDef(object):
         self.is_image = len(self.obs_shape) == 3
         layers = []
         if self.is_image:
+            convs = ((32, 8, 4), (64, 4, 2), (64, 3, 1)) if embedder_scheme is None else \
+                tuple((int(c.num_filters), int(c.kernel_size), int(c.strides)) for c in embedder_scheme)
             h, w, c = self.obs_shape
-            for (n, k, s) in ((32, 8, 4), (64, 4, 2), (64, 3, 1)):
+            for (n, k, s) in convs:
                 conv = Conv2d((h, w), c, n, k, s, "relu")
                 layers.append(conv)
                 h, w, c = conv.OH, conv.OW, n
             flat = h * w * c
         else:
-            layers.append(Dense(self.obs_shape[0], 256, "relu"))
-            flat = 256
+            flat = self.obs_shape[0]
+            for u in ((256,) if embedder_scheme is None else tuple(int(d.units) for d in embedder_scheme)):
+                layers.append(Dense(flat, u, "relu"))
+                flat = u
         for u in self.middleware_units:
             layers.append(Dense(flat, u, "relu"))
             flat = u

@@ -32,7 +32,44 @@ class MiddlewareScheme(object):
 
 class MiddlewareParameters(object):
     def __init__(self, scheme=MiddlewareScheme.Medium):
+        self.scheme = scheme        # a MiddlewareScheme name or a list of Dense specs (fc_middleware.py:56-80)
+
+
+class InputEmbedderParameters(object):
+    """architectures/embedder_parameters.py: scheme "Medium" (the default embedders) or a list of Conv2d / Dense specs"""
+
+    def __init__(self, scheme="Medium"):
         self.scheme = scheme
+
+
+class Conv2d(object):
+    """architectures/layers.py Conv2d(num_filters, kernel_size, strides): one VALID, ReLU convolution of a scheme"""
+
+    def __init__(self, num_filters, kernel_size, strides):
+        self.num_filters, self.kernel_size, self.strides = int(num_filters), int(kernel_size), int(strides)
+
+
+class Dense(object):
+    """architectures/layers.py Dense(units): one ReLU dense layer of a scheme"""
+
+    def __init__(self, units):
+        self.units = int(units)
+
+
+def scheme_layers(scheme):
+    """an embedder scheme as QNetworkDef's embedder_scheme: None for the Medium default, else the list of specs"""
+    if isinstance(scheme, (list, tuple)):
+        return list(scheme)
+    if getattr(scheme, "value", scheme) != "Medium":
+        raise ValueError("embedder scheme %r: only Medium or an explicit layer list is implemented" % (scheme,))
+    return None
+
+
+def middleware_units(scheme):
+    """a middleware scheme as QNetworkDef's middleware_units"""
+    if isinstance(scheme, (list, tuple)):
+        return tuple(d.units for d in scheme)
+    return MiddlewareScheme.units[getattr(scheme, "value", scheme)]
 
 
 class AlgorithmParameters(object):

@@ -199,6 +199,8 @@ def save_checkpoint(agent, checkpoint_dir: str, checkpoint_id: int = 0, env_step
                                                         ("training_iteration", "total_steps_counter",
                                                          "last_target_network_update_step", "last_training_phase_step")
                                                         if hasattr(agent, k)}, "networks": {}}
+    if hasattr(agent, "checkpoint_state"):                    # agent-specific host state (NStepQ: per-stream cuts)
+        meta["agent_state"] = agent.checkpoint_state()
     for tag, store, extra, _ in _network_items(agent):
         base = "%s.net_%s" % (prefix, tag)
         for nm, t in (("theta", store.theta), ("m", store.m), ("v", store.v)):
@@ -254,6 +256,8 @@ def restore_checkpoint(agent, checkpoint_dir: str, name: str = None) -> str:
                 getattr(owner, hook)()
     for k, v in meta["counters"].items():
         setattr(agent, k, v)
+    if "agent_state" in meta:
+        agent.restore_checkpoint_state(meta["agent_state"])
     if getattr(agent, "memory", None) is not None and hasattr(agent.memory, "ring") and \
             os.path.exists(prefix + ".memory.json"):
         restore_memory(agent.memory, prefix)

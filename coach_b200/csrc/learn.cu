@@ -779,6 +779,205 @@ static unsigned flat_grid(int64_t n) {
     return (unsigned)g;
 }
 
+// ---- fused N-step Q head --------------------------------------------------------------------------------------------
+// One warp = one segment (n_step_q_agent.py:99-140): the bootstrap max of the target head, then the segment's rows
+// walked backwards (i = L-1 .. 0) carrying the fp64 return R, and per row Q_online(s), the target, the loss, dL/dQ and
+// the head's backward pass.  Only the taken action's target differs from Q, so dL/dQ is zero off that column: per row
+// one column of dW / db and dh = dq_a W[:, a] relu'(h).  dW / db accumulate in the warp's shared-memory slice ([A][K],
+// lane l owns k = l + 32 j: conflict-free) and leave as per-warp partials for dqn_head_reduce_kernel's fixed-order sum.
+// Lanes hold identical copies of every per-row scalar (the dot products end in an xor butterfly).
+constexpr int kNsMaxA = 18;
+constexpr int kNsWarps = 4;
+
+struct NstepParams {
+    const float *h_online, *h_boot, *w_target, *b_target, *w_online, *b_online;
+    const int64_t* actions;
+    const double* rewards;
+    const uint8_t* game_overs;
+    const int32_t *seg_off, *seg_len;
+    int S, rows, horizon, huber, K, A;
+    double discount;
+    float *q_online, *dq, *targets, *bootstrap, *dh;
+    uint16_t* dh_planes;
+    int64_t dh_plane_stride;
+    float* workspace;
+};
+
+template <int KPL>
+__device__ __forceinline__ void ns_dot(const float* __restrict__ hrow, const float* __restrict__ wt /* smem [A][K] */,
+                                       const float* __restrict__ bias, int A, int K, int lane, float (&hv)[KPL],
+                                       float (&q)[kNsMaxA]) {
+#pragma unroll
+    for (int j = 0; j < KPL; ++j) hv[j] = __ldg(hrow + lane + 32 * j);
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a) {
+        q[a] = 0.f;
+        if (a < A) {
+            float s = 0.f;
+#pragma unroll
+            for (int j = 0; j < KPL; ++j) s = fmaf(hv[j], wt[a * K + lane + 32 * j], s);
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            q[a] = s + __ldg(bias + a);
+        }
+    }
+}
+// np.max over the actions (a NaN propagates)
+__device__ __forceinline__ float ns_max(const float (&q)[kNsMaxA], int A) {
+    float m = q[0];
+#pragma unroll
+    for (int a = 1; a < kNsMaxA; ++a)
+        if (a < A && (q[a] > m || q[a] != q[a])) m = q[a];
+    return m;
+}
+
+template <int KPL>
+__global__ void __launch_bounds__(32 * kNsWarps, 1) nstep_q_head_kernel(NstepParams p) {
+    // Wt_online [A][K] | Wt_target [A][K] | per warp: row buffer [K] | dW [A][K] | db [32]
+    extern __shared__ __align__(16) float ns_smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int gw = blockIdx.x * kNsWarps + warp, nwarps = gridDim.x * kNsWarps;
+    const int A = p.A, K = p.K;
+    float* wt_on = ns_smem;
+    float* wt_tg = ns_smem + A * K;
+    float* rowbuf = ns_smem + 2 * A * K + warp * (K + A * K + 32);
+    float* dwacc = rowbuf + K;
+    float* dbacc = dwacc + A * K;
+    for (int i = threadIdx.x; i < A * K; i += blockDim.x) {               // W [K, A] row-major -> Wt [A][K]
+        const int k = i / A, a = i - k * A;
+        wt_on[a * K + k] = __ldg(p.w_online + i);
+        wt_tg[a * K + k] = __ldg(p.w_target + i);
+    }
+    for (int i = lane; i < A * K + 32; i += 32) dwacc[i] = 0.f;
+    // non-empty segments and the rows they cover (every warp counts them; integer sums are order-free)
+    int nseg = 0, used = 0;
+    for (int s = lane; s < p.S; s += 32) {
+        const int L = p.seg_len[s];
+        if (L > 0) {
+            nseg += 1;
+            used += L;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        nseg += __shfl_xor_sync(0xffffffffu, nseg, o);
+        used += __shfl_xor_sync(0xffffffffu, used, o);
+    }
+    __syncthreads();
+    const float w = nseg > 0 ? 1.0f / (float)nseg : 0.f;                 // the mean over segments
+    float acc_loss = 0.f;
+    if (gw < p.S) {
+        const int s = gw, L = p.seg_len[s], o = p.seg_off[s];
+        const bool valid = L > 0 && o >= 0 && (int64_t)o + L <= p.rows;
+        float hv[KPL], q[kNsMaxA];
+        float boot = 0.f;
+        bool boot_pending = false;
+        if (p.horizon == CB200_NSTEP_NSTEP) {
+            if (valid && !p.game_overs[o + L - 1]) {                       // else R = 0
+                ns_dot<KPL>(p.h_boot + (size_t)s * K, wt_tg, p.b_target, A, K, lane, hv, q);
+                boot = ns_max(q, A);
+                boot_pending = true;
+            }
+            if (p.bootstrap && lane == 0) p.bootstrap[s] = boot;
+        }
+        const float inv_l = valid ? 1.0f / (float)L : 0.f;
+        double R = 0.0;
+        float seg_sum = 0.f;
+        for (int i = (valid ? L : 0) - 1; i >= 0; --i) {
+            const int r = o + i;
+            const int64_t act = p.actions[r];
+            const bool in_range = act >= 0 && act < A;
+            double y = 0.0;
+            bool replace = false;
+            if (p.horizon == CB200_NSTEP_NSTEP) {
+                // R = r_i + discount * R; right after a bootstrap, python float * np.float32 is an fp32 product
+                const double rw = p.rewards[r];
+                R = boot_pending ? __dadd_rn(rw, (double)__fmul_rn((float)p.discount, boot))
+                                 : __dadd_rn(rw, __dmul_rn(p.discount, R));
+                boot_pending = false;
+                y = R;
+                replace = true;
+            } else if (p.horizon == CB200_NSTEP_ONESTEP) {
+                ns_dot<KPL>(p.h_boot + (size_t)r * K, wt_tg, p.b_target, A, K, lane, hv, q);
+                const float qb = ns_max(q, A);
+                if (p.bootstrap && lane == 0) p.bootstrap[r] = qb;
+                y = head_td_target(p.rewards[r], p.game_overs[r], p.discount, qb);
+                replace = true;
+            }
+            ns_dot<KPL>(p.h_online + (size_t)r * K, wt_on, p.b_online, A, K, lane, hv, q);   // hv = h_online slice
+            float qa = 0.f;
+#pragma unroll
+            for (int a = 0; a < kNsMaxA; ++a)
+                if (a == act) qa = q[a];
+            const bool live = replace && in_range;
+            const float ta = (float)y;
+            float dqa = 0.f;
+            if (live) {                                                     // head.py:165-177 on the taken entry
+                const float e = qa - ta;
+                float l, g;
+                if (p.huber) {
+                    const float ae = fabsf(e);
+                    const float qq = fminf(ae, 1.0f);
+                    l = 0.5f * qq * qq + (ae - qq);
+                    g = (ae <= 1.0f) ? e : (e > 0.f ? 1.0f : -1.0f);
+                } else {
+                    l = e * e;
+                    g = 2.0f * e;
+                }
+                seg_sum += l;
+                dqa = w * inv_l * g;
+            }
+            if (lane == 0) {
+#pragma unroll
+                for (int a = 0; a < kNsMaxA; ++a) {
+                    if (a < A) {
+                        const bool here = live && a == act;
+                        p.q_online[(size_t)r * A + a] = q[a];
+                        p.dq[(size_t)r * A + a] = here ? dqa : 0.f;
+                        if (p.targets) p.targets[(size_t)r * A + a] = here ? ta : q[a];
+                    }
+                }
+                if (live) dbacc[act] += dqa;
+            }
+            __syncwarp();                                                   // the previous row's readers are done
+#pragma unroll
+            for (int j = 0; j < KPL; ++j) {
+                const int k = lane + 32 * j;
+                const float wv = live ? wt_on[act * K + k] : 0.f;
+                rowbuf[k] = hv[j] > 0.f ? fmaf(dqa, wv, 0.f) : 0.f;         // relu'(h) on the post-activation value
+                if (live) dwacc[act * K + k] = fmaf(hv[j], dqa, dwacc[act * K + k]);
+            }
+            __syncwarp();
+            head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+        }
+        acc_loss = __fmul_rn(__fmul_rn(seg_sum, inv_l), w);
+    }
+    // padding rows [used, rows): zero Q, dq, targets, dh
+    for (int r = used + gw; r < p.rows; r += nwarps) {
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) rowbuf[lane + 32 * j] = 0.f;
+        for (int a = lane; a < A; a += 32) {
+            p.q_online[(size_t)r * A + a] = 0.f;
+            p.dq[(size_t)r * A + a] = 0.f;
+            if (p.targets) p.targets[(size_t)r * A + a] = 0.f;
+        }
+        if (p.horizon == CB200_NSTEP_ONESTEP && p.bootstrap && lane == 0) p.bootstrap[r] = 0.f;
+        __syncwarp();
+        head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+    }
+    __syncwarp();
+    // per-warp partials in dqn_head_reduce_kernel's layout: [dW (K * A) | db (A) | loss (1)]
+    float* part = p.workspace + (size_t)gw * ((size_t)K * A + A + 1);
+#pragma unroll
+    for (int j = 0; j < KPL; ++j)
+        for (int a = 0; a < A; ++a) part[((size_t)lane + 32 * j) * A + a] = dwacc[a * K + lane + 32 * j];
+    if (lane == 0) {
+        for (int a = 0; a < A; ++a) part[(size_t)K * A + a] = dbacc[a];
+        part[(size_t)K * A + A] = acc_loss;
+    }
+}
+
 }  // namespace cb200
 
 using namespace cb200;
@@ -910,6 +1109,61 @@ int cb200_ensemble_head_fused(const cb200_ensemble_head_desc* d, void* stream) {
     CB200_LAUNCH(ensemble_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, p.workspace, nparts, n_out,
                  p.K * p.A, p.A, p.H * p.A, 1.0f / (float)p.B, d->dw, d->db, d->losses);
     if (d->loss) CB200_LAUNCH(ensemble_loss_total_kernel, 1, 1, 0, st, d->losses, p.H, d->loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_nstep_q_head(const cb200_nstep_q_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->horizon >= CB200_NSTEP_NONE && d->horizon <= CB200_NSTEP_ONESTEP, "unknown horizon");
+    CB200_CHECK_ARG(d->h_online && (d->horizon == CB200_NSTEP_NONE || d->h_boot) && d->w_target && d->b_target &&
+                        d->w_online && d->b_online && d->actions && d->rewards && d->game_overs && d->seg_offsets &&
+                        d->seg_lengths && d->q_online && d->dq && d->dw && d->db && d->workspace,
+                    "null pointer");
+    CB200_CHECK_ARG(d->segments >= 1 && d->segments <= (1 << 20), "1 <= segments <= 2^20");
+    CB200_CHECK_ARG(d->rows >= 1 && d->rows <= (1 << 24), "1 <= rows <= 2^24");
+    CB200_CHECK_ARG(d->n_actions >= 1 && d->n_actions <= kNsMaxA, "1 <= n_actions <= 18");
+    CB200_CHECK_ARG(d->features == 256 || d->features == 512, "features must be 256 or 512");
+    CB200_CHECK_ARG(!d->dh_planes || (d->dh_plane_stride % 8 == 0 && d->rows % 8 == 0), "planes: rows % 8, stride % 8");
+    NstepParams p;
+    p.h_online = d->h_online; p.h_boot = d->h_boot;
+    p.w_target = d->w_target; p.b_target = d->b_target; p.w_online = d->w_online; p.b_online = d->b_online;
+    p.actions = d->actions; p.rewards = d->rewards; p.game_overs = d->game_overs;
+    p.seg_off = d->seg_offsets; p.seg_len = d->seg_lengths;
+    p.S = d->segments; p.rows = (int)d->rows; p.horizon = d->horizon; p.huber = d->huber;
+    p.K = d->features; p.A = d->n_actions; p.discount = d->discount;
+    p.q_online = d->q_online; p.dq = d->dq; p.targets = d->targets; p.bootstrap = d->bootstrap; p.dh = d->dh;
+    p.dh_planes = static_cast<uint16_t*>(d->dh_planes); p.dh_plane_stride = d->dh_plane_stride;
+    p.workspace = d->workspace;
+    const unsigned grid = (unsigned)((p.S + kNsWarps - 1) / kNsWarps);
+    const int nparts = (int)grid * kNsWarps;                   // idle warps write zero partials
+    cudaStream_t st = as_stream(stream);
+    // up to 225 KB at K = 512, A = 18 (two staged kernels and four warps' dW slices): opted into once per instantiation
+    // and device, at the size of the largest shape
+    auto smem_of = [](int A, int K) { return (size_t)(2 * A * K + kNsWarps * (K + A * K + 32)) * sizeof(float); };
+    const size_t smem = smem_of(p.A, p.K);
+    static bool attr_set[kMaxDevices][2] = {};
+    int dev = 0;
+    CB200_CUDA(cudaGetDevice(&dev));
+    CB200_CHECK_ARG(dev < kMaxDevices, "device ordinal out of range");
+    const int ti = p.K == 512 ? 1 : 0;
+    if (!attr_set[dev][ti]) {
+        if (ti)
+            CB200_CUDA(cudaFuncSetAttribute(nstep_q_head_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem_of(kNsMaxA, 512)));
+        else
+            CB200_CUDA(cudaFuncSetAttribute(nstep_q_head_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem_of(kNsMaxA, 256)));
+        attr_set[dev][ti] = true;
+    }
+    if (p.K == 512) {
+        CB200_LAUNCH(nstep_q_head_kernel<16>, grid, 32 * kNsWarps, smem, st, p);
+    } else {
+        CB200_LAUNCH(nstep_q_head_kernel<8>, grid, 32 * kNsWarps, smem, st, p);
+    }
+    const int n_out = p.K * p.A + p.A + 1;
+    CB200_LAUNCH(dqn_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, p.workspace, nparts, n_out,
+                 p.K * p.A, p.A, 1.0f, d->dw, d->db, d->loss);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

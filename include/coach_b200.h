@@ -477,6 +477,62 @@ typedef struct cb200_ensemble_head_desc {
 
 int cb200_ensemble_head_fused(const cb200_ensemble_head_desc* e_desc, void* stream);
 
+/* Fused N-step Q head (agents/n_step_q_agent.py:99-140): a plain QHead Dense(n_actions) on one feature layer, trained
+ * on on-policy segments.  Segment s covers the rows [seg_offsets[s], seg_offsets[s] + seg_lengths[s]); a slot with
+ * length 0 is unused.  The non-empty segments must be disjoint and together cover rows [0, n), n = the sum of the
+ * lengths <= rows; rows [n, rows) are padding and get zero dq, dh and targets.  With S non-empty segments, per row i of a
+ * segment of length L:
+ *   targets[i] = Q_online(s_i) with the taken action's entry replaced by
+ *     NSTEP (N-Step): R_i, walking i = L-1 .. 0 with R = r_i + discount R, in fp64.  R starts at 0 when the segment's
+ *       last game_over is set, else at B = max_a Q_target(h_boot[s]) (fp32).  The first step after a bootstrap is
+ *       numpy's python float * np.float32: (float)discount * B is rounded in fp32, then added to r_i in fp64.
+ *     ONESTEP (1-Step): r_i + ((1 - done_i) discount) max_a Q_target(h_boot[i]), fp64 (as cb200_dqn_head_fused).
+ *     NONE: nothing is replaced (the reference's fall-through): the loss and every gradient are 0.
+ *   Every operation is an explicit _rn intrinsic; a row whose action is outside [0, n_actions) keeps Q(s).
+ *   loss = (1/S) sum_s (1/L_s) sum_{i in s} sum_a l(Q - target), l Huber (delta 1) or squared error;
+ *   dq = (1/S) (1/L_s) l'(Q - target), then dW = h^T dq, db = sum_i dq_i and dh = (dq W^T) relu'(h), as
+ *   cb200_dqn_head_fused produces them.  features 256 or 512, n_actions <= 18.  Deterministic: per-warp partials reduced
+ *   in a fixed order by a second launch, no atomics; repeat calls and graph replays give the same bits. */
+typedef struct cb200_nstep_q_head_desc {
+    const float* h_online;      /* [rows, features] post-ReLU features of s from the online network                      */
+    const float* h_boot;        /* TARGET-network features: NSTEP [segments, features] of each segment's last s';
+                                   ONESTEP [rows, features] of every row's s'; unused for NONE                            */
+    const float* w_target;      /* target head kernel [features, n_actions] and bias                                      */
+    const float* b_target;
+    const float* w_online;
+    const float* b_online;
+    const int64_t* actions;     /* [rows]                                                                                 */
+    const double* rewards;      /* [rows]                                                                                 */
+    const uint8_t* game_overs;  /* [rows]                                                                                 */
+    const int32_t* seg_offsets; /* [segments]                                                                             */
+    const int32_t* seg_lengths; /* [segments], 0 = unused slot                                                           */
+    int32_t segments;           /* slots in the table, 1 .. 2^20                                                         */
+    int64_t rows;               /* rows of the feature / output buffers, 1 .. 2^24                                       */
+    double discount;
+    int32_t horizon;            /* CB200_NSTEP_*                                                                         */
+    int32_t huber;              /* 1: tf.losses.huber_loss(delta 1), 0: mean squared error                                */
+    int32_t features;           /* 256 or 512                                                                             */
+    int32_t n_actions;          /* 1 .. 18                                                                                */
+    float* q_online;            /* out [rows, n_actions]                                                                  */
+    float* dq;                  /* out [rows, n_actions]: dL/dQ                                                           */
+    float* loss;                /* out scalar, optional                                                                   */
+    float* targets;             /* out, optional [rows, n_actions]                                                        */
+    float* bootstrap;           /* out, optional: NSTEP [segments] B (0 for a terminal or unused segment);
+                                   ONESTEP [rows] max_a Q_target(s'_i) (0 for padding rows)                               */
+    float* dh;                  /* out, optional: [rows, features] dL/d(pre-activation of the feature layer)             */
+    void* dh_planes;            /* out, optional: the same as tiled bf16 hi / mid / lo planes                             */
+    int64_t dh_plane_stride;
+    float* dw;                  /* out [features, n_actions]                                                              */
+    float* db;                  /* out [n_actions]                                                                        */
+    float* workspace;           /* ceil(segments / 4) * 4 * (features * n_actions + n_actions + 1) floats                */
+} cb200_nstep_q_head_desc;
+
+#define CB200_NSTEP_NONE 0
+#define CB200_NSTEP_NSTEP 1
+#define CB200_NSTEP_ONESTEP 2
+
+int cb200_nstep_q_head(const cb200_nstep_q_head_desc* n_desc, void* stream);
+
 /* Acting values of an ensemble, q [envs, heads * n_actions] -> out [envs, n_actions], in the exploration policies' fp32
  * numpy arithmetic (exploration_policies/bootstrapped.py:70-84, ucb.py:70-83):
  *   SELECT  the row of head[e] (Bootstrapped, training)
