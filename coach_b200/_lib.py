@@ -115,6 +115,23 @@ class NstepQHeadDesc(ctypes.Structure):
 NSTEP_NONE, NSTEP_NSTEP, NSTEP_ONESTEP = 0, 1, 2
 
 
+class ActorCriticHeadDesc(ctypes.Structure):
+    """struct cb200_actor_critic_head_desc"""
+    _fields_ = [("h", c_void_p), ("h_boot", c_void_p), ("w", c_void_p), ("b", c_void_p), ("actions", c_void_p),
+                ("rewards", c_void_p), ("game_overs", c_void_p), ("seg_offsets", c_void_p), ("seg_lengths", c_void_p),
+                ("segments", ctypes.c_int32), ("rows", c_i64), ("discount", c_double), ("gae_lambda", c_double),
+                ("mode", ctypes.c_int32), ("huber", ctypes.c_int32), ("beta_entropy", c_float),
+                ("v_weight", c_float), ("p_weight", c_float), ("features", ctypes.c_int32),
+                ("n_actions", ctypes.c_int32), ("z", c_void_p), ("dz", c_void_p), ("loss", c_void_p),
+                ("probs", c_void_p), ("targets", c_void_p), ("advantages", c_void_p), ("bootstrap", c_void_p),
+                ("dh", c_void_p), ("dh_planes", c_void_p), ("dh_plane_stride", c_i64), ("dw", c_void_p),
+                ("db", c_void_p), ("workspace", c_void_p)]
+
+
+# cb200_actor_critic_head_desc.mode
+AC_A_VALUE, AC_GAE, AC_GAE_VALUE = 0, 1, 2
+
+
 # cb200_ensemble_action_values modes
 ENSEMBLE_SELECT, ENSEMBLE_UCB, ENSEMBLE_MEAN, ENSEMBLE_VOTE = 0, 1, 2, 3
 
@@ -170,6 +187,8 @@ PROTOTYPES = {
     "cb200_dqn_head_fused": (c_int, [c_void_p, c_void_p]),
     "cb200_ensemble_head_fused": (c_int, [c_void_p, c_void_p]),
     "cb200_nstep_q_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_actor_critic_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_categorical_act": (c_int, [c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "cb200_ensemble_action_values": (c_int, [c_void_p, c_i64, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, c_void_p,
                                              c_float, c_void_p, c_void_p]),
     "cb200_dueling_combine_fwd": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p, c_void_p]),

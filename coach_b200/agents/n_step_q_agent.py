@@ -11,16 +11,12 @@ segments of each segment's own gradient (the synchronous-training rule of
 lock-step steps (each stream's own steps); ``training_iteration`` counts learn steps.  With E = 1 this is the
 reference schedule.
 
-Device rollout buffer: t_max slots per stream, slot (t mod t_max) * E + e for stream e at lock-step t: a segment spans at
-most t_max consecutive steps and is consumed at the step it closes, so a slot is never overwritten while it is live.
-``observe_batch`` stores one lock-step with one host-to-device copy per column and one ring scatter; ``train`` gathers
-the closed segments' rows (and their bootstrap states) into the learn buffers with ``cb200_gather``.
+The rollout buffer, the cuts, the gather and the 32-row buckets with their CUDA graphs are
+``coach_b200.memories.lockstep_segments``.
 
 One learn step = gather -> target features of the bootstrap states (N-Step) or of every s' (1-Step) -> online features
 -> ``cb200_nstep_q_head`` (Q, bootstrap max, the fp64 return recurrence, targets, loss, dL/dQ, the head's gradients and
-dL/dh) -> backward -> TF-Adam.  Rows are rounded up to a multiple of 32 (padding rows carry no weight) and every such
-bucket has its own forward / backward instance on the shared parameters; from 128 rows on each bucket's step is
-replayed as one CUDA graph.
+dL/dh) -> backward -> TF-Adam.  Every 32-row bucket has its own forward / backward instance on the shared parameters.
 
 Refused (ValueError): ``apply_gradients_every_x_episodes != 1`` (gradients are applied after every segment), a
 ``targets_horizon`` other than 'N-Step' / '1-Step' (the reference silently trains on zero loss then), a dueling head, and
@@ -40,6 +36,7 @@ from coach_b200.architectures.q_network import QNetworkDef
 from coach_b200.base_parameters import (AgentParameters, AlgorithmParameters, EnvironmentSteps,
                                         InputEmbedderParameters, NetworkParameters, middleware_units, scheme_layers)
 from coach_b200.exploration_policies.e_greedy import EGreedyParameters
+from coach_b200.memories.lockstep_segments import LockstepSegments
 
 HORIZONS = {"N-Step": _lib.NSTEP_NSTEP, "1-Step": _lib.NSTEP_ONESTEP}
 
@@ -81,10 +78,6 @@ class NStepQAgentParameters(AgentParameters):
         return 'coach_b200.agents.n_step_q_agent:NStepQAgent'
 
 
-def _round32(n):
-    return max(32, (int(n) + 31) // 32 * 32)
-
-
 class NStepQAgent(object):
     def __init__(self, agent_parameters, parent=None, observation_shape=None, num_actions=None, num_envs=1,
                  device=None, seed=None):
@@ -106,36 +99,16 @@ class NStepQAgent(object):
                                              else ap.observation_shape)
         self.num_actions = A = int(num_actions if num_actions is not None else ap.num_actions)
         self.num_envs = E = int(num_envs)
-        self.t_max = T = int(alg.num_steps_between_gradient_updates)
-        if E < 1 or T < 1:
-            raise ValueError("num_envs and num_steps_between_gradient_updates must be >= 1")
+        self.t_max = int(alg.num_steps_between_gradient_updates)
         self.horizon = HORIZONS[alg.targets_horizon]
-        obs_dtype = torch.uint8 if len(obs) == 3 else torch.float32
         emb = getattr(net_params, "input_embedders_parameters", {}).get("observation")
         scheme = getattr(getattr(net_params, "middleware_parameters", None), "scheme", "Medium")
         self.net_def = QNetworkDef(dev, obs, A, middleware_units=middleware_units(scheme),
                                    embedder_scheme=scheme_layers(getattr(emb, "scheme", "Medium")))
         gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
         self.net_def.store.init_glorot(gen)
-        # rollout buffer: [t_max * E] rows per column, slot (t % t_max) * E + e
-        z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)        # noqa: E731
-        self.rollout = {"state": z((T * E,) + obs, obs_dtype), "next_state": z((T * E,) + obs, obs_dtype),
-                        "action": z(T * E, torch.int64), "reward": z(T * E, torch.float64),
-                        "game_over": z(T * E, torch.uint8)}
-        self._stage_dev = {k: torch.zeros((E,) + tuple(v.shape[1:]), dtype=v.dtype, device=dev)
-                           for k, v in self.rollout.items()}
-        pin = dev.type == "cuda"
-        self._stage_host = {k: torch.zeros(v.shape, dtype=v.dtype, pin_memory=pin) for k, v in self._stage_dev.items()}
-        self._stage_ev = None
-        # learn buffers: at most E * t_max rows close at one step
-        self.max_rows = R = _round32(E * T)
-        self.learn = {k: z((R,) + tuple(v.shape[1:]), v.dtype) for k, v in self.rollout.items()}
-        self.boot_states = z((E,) + obs, obs_dtype)
-        self._idx_dev = z(R + E, torch.int64)                     # row slots | bootstrap slots
-        self._seg_dev = z(2 * E, torch.int32)                     # offsets | lengths
-        self._idx_host = torch.zeros(R + E, dtype=torch.int64, pin_memory=pin)
-        self._seg_host = torch.zeros(2 * E, dtype=torch.int32, pin_memory=pin)
-        self._tab_ev = None
+        self.segments = sg = LockstepSegments(self.lib, dev, obs, E, self.t_max)
+        self.learn, self.boot_states, self.max_rows = sg.learn, sg.boot_states, sg.max_rows
         # the shared parameters (online, target, Adam) and the acting path of the DQN agent.  The wrapper's own
         # bindings are the 32-row bucket.
         self.batch_buffers = {"state:observation": self.learn["state"][:32],
@@ -150,22 +123,13 @@ class NStepQAgent(object):
                                                         net.theta_target)
             net.add_planes(self.target_boot)
         self._buckets = {}
-        self._graphs = {}
-        self._eager = {}
-        self.loss_dev = z(1, torch.float32)
-        self._fetch_host = torch.zeros(2, dtype=torch.float32, pin_memory=pin)
-        self.graph_kernel_launches = 0
+        self.loss_dev = torch.zeros(1, dtype=torch.float32, device=dev)
+        self._fetch_host = torch.zeros(2, dtype=torch.float32, pin_memory=dev.type == "cuda")
         self._acting = {}
-        # counters of agents/agent.py:112-135 and the per-stream cut state of policy_optimization_agent.py:85-135
+        # counters of agents/agent.py:112-135
         self.training_iteration = 0
         self.total_steps_counter = 0
         self.last_target_network_update_step = 0
-        self._t = 0                                            # lock-steps observed
-        self.episode_length = np.zeros(E, dtype=np.int64)
-        self.last_gradient_update_step_idx = np.zeros(E, dtype=np.int64)
-        self.complete = np.zeros(E, dtype=bool)
-        self.segment_start = np.zeros(E, dtype=np.int64)       # lock-step of the open segment's first stored row
-        self.learned_segments = []                             # (stream, start, end) of the last train() step
 
     # ---- reference plumbing and the DQN agent's acting path -------------------------------------------------------------
     @property
@@ -179,44 +143,21 @@ class NStepQAgent(object):
     def _join_optimizer(self):
         pass                                                   # the optimizer runs on the caller's stream
 
+    @property
+    def learned_segments(self):
+        """(stream, start, end) of the segments the last train() step learned"""
+        return self.segments.learned_segments
+
+    @property
+    def graph_kernel_launches(self):
+        return self.segments.graph_kernel_launches
+
     # ---- rollout ----------------------------------------------------------------------------------------------------------
     def observe_batch(self, states, actions, rewards, next_states, game_overs):
         """one lock-step of the E streams (agent.py:820-834 act's step count, :905-975 observe, core_types.py:716-725
         Episode.insert): host arrays [E, ...]"""
-        E, T = self.num_envs, self.t_max
-        cols = {"state": states, "next_state": next_states, "action": actions, "reward": rewards,
-                "game_over": game_overs}
-        if self._stage_ev is not None:
-            self._stage_ev.synchronize()                       # the previous step's copies have left the staging
-        for k, v in cols.items():
-            h = self._stage_host[k]
-            h.numpy()[...] = np.asarray(v).reshape(h.shape)
-            self._stage_dev[k].copy_(h, non_blocking=True)
-        self._stage_ev = torch.cuda.Event()
-        self._stage_ev.record()
-        arr, n = _lib.make_columns((self.rollout[k].data_ptr(), self._stage_dev[k].data_ptr(),
-                                    self.rollout[k][0].numel() * self.rollout[k].element_size())
-                                   for k in ("state", "next_state", "action", "reward", "game_over"))
-        _lib.check(self.lib.cb200_scatter_ring(arr, n, (self._t % T) * E, T * E, E, _lib.current_stream()))
+        self.segments.observe(states, actions, rewards, next_states, game_overs)
         self.total_steps_counter += 1
-        self._t += 1
-        self.episode_length += 1
-        self.complete |= np.asarray(game_overs).reshape(E).astype(bool)
-
-    def _close_segments(self):
-        """policy_optimization_agent.py:88-110 for every stream: (streams, rows) of the segments closed now"""
-        passed = self.episode_length - self.last_gradient_update_step_idx
-        closes = (passed >= self.t_max) | self.complete
-        streams = np.nonzero(closes)[0]
-        rows = np.minimum(passed, self._t - self.segment_start)[streams]
-        self.learned_segments = [(int(e), int(self.last_gradient_update_step_idx[e]), int(self.episode_length[e]))
-                                 for e in streams]
-        self.last_gradient_update_step_idx[streams] = np.where(self.complete[streams], 0, self.episode_length[streams])
-        self.episode_length[self.complete] = 0
-        self.complete[:] = False
-        self.segment_start[streams] = self._t
-        keep = rows > 0
-        return streams[keep], rows[keep]
 
     def train(self, fetch=True):
         """n_step_q_agent.py:142-153 + policy_optimization_agent.py:85-135: target copy check first, then one learn step
@@ -224,32 +165,11 @@ class NStepQAgent(object):
         net = self.networks["main"]
         if self._should_update_online_weights_to_target():
             net.update_target_network(self.ap.algorithm.rate_for_copying_weights_to_target)
-        streams, rows = self._close_segments()
+        streams, rows = self.segments.close()
         if len(streams) == 0:
             return 0
         self.training_iteration += 1
-        E, T, t_last = self.num_envs, self.t_max, self._t - 1
-        n = int(rows.sum())
-        B = _round32(n)
-        offsets = np.concatenate([[0], np.cumsum(rows)[:-1]]).astype(np.int64)
-        # row j of segment s is the lock-step t_last - rows[s] + 1 + j of its stream
-        seg_of_row = np.repeat(np.arange(len(streams)), rows)
-        j = np.arange(n) - offsets[seg_of_row]
-        steps = t_last - rows[seg_of_row] + 1 + j
-        if self._tab_ev is not None:
-            self._tab_ev.synchronize()
-        idx, seg = self._idx_host.numpy(), self._seg_host.numpy()
-        idx[:] = 0
-        idx[:n] = (steps % T) * E + streams[seg_of_row]
-        idx[self.max_rows:self.max_rows + len(streams)] = (t_last % T) * E + streams
-        seg[:] = 0
-        seg[:len(streams)] = offsets
-        seg[E:E + len(streams)] = rows
-        self._idx_dev.copy_(self._idx_host, non_blocking=True)
-        self._seg_dev.copy_(self._seg_host, non_blocking=True)
-        self._tab_ev = torch.cuda.Event()
-        self._tab_ev.record()
-        return self._learn(B, True, fetch)
+        return self._learn(self.segments.tables(streams, rows), True, fetch)
 
     # ---- the learn step ---------------------------------------------------------------------------------------------------
     def learn_from_batch(self, batch, fetch=True):
@@ -257,24 +177,8 @@ class NStepQAgent(object):
         states / next_states / actions / rewards / game_overs over the rows, and "lengths": the segments' lengths in row
         order (at most num_envs of them).  Returns (loss, [loss], unclipped gradient norm) with fetch, else device
         scalars."""
-        lengths = np.asarray(batch["lengths"], dtype=np.int64)
-        n, S = int(lengths.sum()), len(lengths)
-        if S < 1 or S > self.num_envs or n > self.max_rows or (lengths < 1).any():
-            raise ValueError("1..num_envs segments of >= 1 rows, at most num_envs * t_max rows in total")
-        for k, key in (("state", "states"), ("next_state", "next_states"), ("action", "actions"),
-                       ("reward", "rewards"), ("game_over", "game_overs")):
-            self.learn[k][:n].copy_(torch.as_tensor(np.ascontiguousarray(batch[key])).reshape(
-                self.learn[k][:n].shape))
-        if self.horizon == _lib.NSTEP_NSTEP:
-            last = np.cumsum(lengths) - 1
-            self.boot_states.zero_()
-            self.boot_states[:S].copy_(torch.as_tensor(np.ascontiguousarray(np.asarray(batch["next_states"])[last]))
-                                       .reshape(self.boot_states[:S].shape))
-        seg = np.zeros(2 * self.num_envs, dtype=np.int32)
-        seg[:S] = np.concatenate([[0], np.cumsum(lengths)[:-1]])
-        seg[self.num_envs:self.num_envs + S] = lengths
-        self._seg_dev.copy_(torch.from_numpy(seg))
-        return self._learn(_round32(n), False, fetch)
+        B = self.segments.load(batch, boot=self.horizon == _lib.NSTEP_NSTEP)
+        return self._learn(B, False, fetch)
 
     def _bucket(self, B):
         bk = self._buckets.get(B)
@@ -308,7 +212,7 @@ class NStepQAgent(object):
         d.w_online, d.b_online = store.view(net.theta, wname).data_ptr(), store.view(net.theta, bname).data_ptr()
         d.actions, d.rewards = self.learn["action"].data_ptr(), self.learn["reward"].data_ptr()
         d.game_overs = self.learn["game_over"].data_ptr()
-        d.seg_offsets, d.seg_lengths = self._seg_dev.data_ptr(), self._seg_dev.data_ptr() + 4 * E
+        d.seg_offsets, d.seg_lengths = self.segments.seg_table()
         d.segments, d.rows = E, B
         d.discount = float(self.ap.algorithm.discount)
         d.horizon = self.horizon
@@ -332,13 +236,7 @@ class NStepQAgent(object):
         if gather:
             keys = ("state", "action", "reward", "game_over") + \
                 (("next_state",) if self.horizon == _lib.NSTEP_ONESTEP else ())
-            arr, n = _lib.make_columns((self.rollout[k].data_ptr(), self.learn[k].data_ptr(),
-                                        self.rollout[k][0].numel() * self.rollout[k].element_size()) for k in keys)
-            _lib.check(lib.cb200_gather(arr, n, self._idx_dev.data_ptr(), B, st))
-            if self.horizon == _lib.NSTEP_NSTEP:
-                arr, n = _lib.make_columns([(self.rollout["next_state"].data_ptr(), self.boot_states.data_ptr(),
-                                             self.boot_states[0].numel() * self.boot_states.element_size())])
-                _lib.check(lib.cb200_gather(arr, n, self._idx_dev.data_ptr() + 8 * self.max_rows, self.num_envs, st))
+            self.segments.gather(B, keys, self.horizon == _lib.NSTEP_NSTEP, st)
         if on.theta_planes is not None and on is not net.online_s:
             on.theta_planes.refresh()                          # this bucket's operand planes of the current theta
         tn.forward_features()
@@ -355,20 +253,7 @@ class NStepQAgent(object):
         net.apply_gradients(1.0)
 
     def _learn(self, B, gather, fetch):
-        graph = gather and B >= 128 and self.device.type == "cuda" and _lib.tune_default("nstep_graph", 1)
-        if graph and self._eager.get(B, 0) >= 2:
-            g = self._graphs.get(B)
-            if g is None:
-                c0 = self.lib.cb200_launch_count()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._device_step(B, gather)
-                g = self._graphs[B] = (g, int(self.lib.cb200_launch_count() - c0))
-            g[0].replay()
-            self.graph_kernel_launches += g[1]
-        else:
-            self._device_step(B, gather)
-            self._eager[B] = self._eager.get(B, 0) + 1
+        self.segments.run(B, gather, self._device_step, _lib.tune_default("nstep_graph", 1))
         if not fetch:
             return self.loss_dev if gather else (self.loss_dev, [self.loss_dev], self.networks["main"].sumsq)
         self._fetch_host[0:1].copy_(self.loss_dev, non_blocking=True)
@@ -382,13 +267,7 @@ class NStepQAgent(object):
     # ---- checkpoints (coach_b200/checkpoint.py) -------------------------------------------------------------------------
     def checkpoint_state(self):
         """every stream's cut position; the rows of open segments are not saved"""
-        return {"t": int(self._t), "episode_length": self.episode_length.tolist(),
-                "last_gradient_update_step_idx": self.last_gradient_update_step_idx.tolist(),
-                "complete": self.complete.tolist()}
+        return self.segments.state()
 
     def restore_checkpoint_state(self, state):
-        self._t = int(state["t"])
-        self.episode_length[:] = state["episode_length"]
-        self.last_gradient_update_step_idx[:] = state["last_gradient_update_step_idx"]
-        self.complete[:] = state["complete"]
-        self.segment_start[:] = self._t                        # nothing of the open segments is in the buffer
+        self.segments.restore(state)

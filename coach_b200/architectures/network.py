@@ -27,6 +27,7 @@ class ParamStore(object):
         self.theta = None
         self.glorot_fans = {}             # kernel name -> (fan_in, fan_out) when it is not the tensor's own
         self.initial_values = {}          # rescaler name -> initial value (default 1.0)
+        self.normalized_columns = {}      # kernel name -> (first n columns, std): normalized_columns_initializer
 
     def add(self, name, shape):
         if self.theta is not None:
@@ -69,6 +70,10 @@ class ParamStore(object):
                 fan_in, fan_out = self.glorot_fans.get(name, (fan_in, fan_out))
                 limit = float(np.sqrt(6.0 / (fan_in + fan_out)))
                 cpu = (torch.rand(shape, generator=generator, dtype=torch.float32) * 2 - 1) * limit
+                if name in self.normalized_columns:          # head.py:28-33: randn scaled to a column norm of std
+                    n, std = self.normalized_columns[name]
+                    w = torch.randn((shape[0], n), generator=generator, dtype=torch.float32)
+                    cpu[:, :n] = w * (std / torch.sqrt((w * w).sum(dim=0, keepdim=True)))
                 v.copy_(cpu)
             elif name.endswith("rescalers"):
                 v.fill_(self.initial_values.get(name, 1.0))

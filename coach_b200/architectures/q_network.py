@@ -10,6 +10,9 @@ Structure and variable order follow the TF graph of the reference:
                DuelingQHead: V: Dense(512) ReLU, Dense(1); A: Dense(512) ReLU, Dense(num_actions);
                Q = V + (A - mean_a A) (dueling_q_head.py:33-47)
   + one scalar ``gradients_from_head_0-0_rescalers`` variable (general_network.py:312-315; gradient identically 0)
+
+With ``value_head`` the heads are the actor-critic pair VHead + PolicyHead (actor_critic_agent.py:66-70) as ONE
+Dense(1 + num_actions): column 0 is V, columns 1..num_actions the policy logits.
 """
 import numpy as np
 import torch
@@ -24,7 +27,7 @@ class QNetworkDef(object):
     """Parameter layout + layer chain; instances bind it to buffers (see QNetworkInstance)."""
 
     def __init__(self, device, observation_shape, num_actions, dueling=False, embedder="auto", middleware_units=512,
-                 head_copies=1, head_grad_rescale=1.0, embedder_scheme=None):
+                 head_copies=1, head_grad_rescale=1.0, embedder_scheme=None, value_head=False):
         """embedder_scheme: the input embedder's layers (InputEmbedderParameters.scheme as a list): for images a list of
         base_parameters.Conv2d specs, for vectors a list of base_parameters.Dense specs; None is the Medium embedder
         above (image_embedder.py:62-67 / vector_embedder.py:58-61).
@@ -33,7 +36,14 @@ class QNetworkDef(object):
         outputs on the same features, as ONE Dense(head_copies * num_actions) whose column block [k A, (k + 1) A) is
         head k; each block is Glorot-initialised with the fans of its own [F, A] layer, and there is one
         ``gradients_from_head_0-<k>_rescalers`` scalar per copy, initialised to ``head_grad_rescale``
-        (general_network.py:304-325)."""
+        (general_network.py:304-325).
+        value_head (ActorCritic): VHead Dense(1) + PolicyHead Dense(num_actions) as ONE Dense(1 + num_actions); column 0
+        is initialised as normalized_columns_initializer(1.0) (v_head.py:44-47, head.py:28-33), the policy block
+        Glorot-uniform with the fans of its own [F, num_actions] layer; one ``gradients_from_head_{0,1}-0_rescalers``
+        scalar per head."""
+        self.value_head = bool(value_head)
+        if self.value_head and (dueling or head_copies != 1):
+            raise NotImplementedError("the actor-critic head takes neither a dueling head nor head copies")
         self.head_copies = int(head_copies)
         self.head_grad_rescale = float(head_grad_rescale)
         if self.head_copies > 1 and dueling:
@@ -69,18 +79,23 @@ class QNetworkDef(object):
             flat = u
         middleware_units = flat                 # width of what the head reads
         if not self.dueling:
-            layers.append(Dense(middleware_units, self.head_copies * self.num_actions, None))
+            layers.append(Dense(middleware_units, self.head_copies * self.num_actions + self.value_head, None))
             self.trunk = Sequential(layers, self.store, "main/online/network_0")
             self.v_tower = self.a_tower = None
-            if self.head_copies > 1:
+            if self.head_copies > 1 or self.value_head:
                 self.store.glorot_fans[self.trunk.names[-1][0]] = (middleware_units, self.num_actions)
+            if self.value_head:
+                self.store.normalized_columns[self.trunk.names[-1][0]] = (1, 1.0)
         else:
             self.trunk = Sequential(layers, self.store, "main/online/network_0")
             self.v_tower = Sequential([Dense(middleware_units, 512, "relu"), Dense(512, 1, None)], self.store,
                                       "main/online/network_0/dueling_q_values_head_0/state_value")
             self.a_tower = Sequential([Dense(middleware_units, 512, "relu"), Dense(512, self.num_actions, None)],
                                       self.store, "main/online/network_0/dueling_q_values_head_0/action_advantage")
-        if self.head_copies == 1:
+        if self.value_head:
+            for k in range(2):
+                self.store.add("main/online/network_0/gradients_from_head_%d-0_rescalers" % k, ())
+        elif self.head_copies == 1:
             self.store.add("main/online/network_0/gradients_from_head_0-0_rescalers", ())
         else:
             for k in range(self.head_copies):

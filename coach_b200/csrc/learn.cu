@@ -803,14 +803,14 @@ struct NstepParams {
     float* workspace;
 };
 
-template <int KPL>
+template <int KPL, int MAXA = kNsMaxA>
 __device__ __forceinline__ void ns_dot(const float* __restrict__ hrow, const float* __restrict__ wt /* smem [A][K] */,
                                        const float* __restrict__ bias, int A, int K, int lane, float (&hv)[KPL],
-                                       float (&q)[kNsMaxA]) {
+                                       float (&q)[MAXA]) {
 #pragma unroll
     for (int j = 0; j < KPL; ++j) hv[j] = __ldg(hrow + lane + 32 * j);
 #pragma unroll
-    for (int a = 0; a < kNsMaxA; ++a) {
+    for (int a = 0; a < MAXA; ++a) {
         q[a] = 0.f;
         if (a < A) {
             float s = 0.f;
@@ -975,6 +975,288 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) nstep_q_head_kernel(NstepPar
     if (lane == 0) {
         for (int a = 0; a < A; ++a) part[(size_t)K * A + a] = dbacc[a];
         part[(size_t)K * A + A] = acc_loss;
+    }
+}
+
+// ---- fused actor-critic (A3C) head ----------------------------------------------------------------------------------
+// One Dense(1 + A) on the feature layer: column 0 is the VHead, columns 1..A the PolicyHead logits.  One warp = one
+// segment (actor_critic_agent.py:111-165), the segment table and the conventions of nstep_q_head_kernel: V of each
+// segment's last s' (the online network: the reference bootstraps with online_network.predict), the rows walked
+// backwards carrying the A_VALUE return or the GAE recurrences in fp64 in numpy's / scipy.signal.lfilter's operation
+// order, then per row the softmax, the three loss terms and a dense dL/dZ over all 1 + A columns.  dW / db accumulate in
+// the warp's shared-memory slice and leave as per-warp partials for dqn_head_reduce_kernel's fixed-order sum.
+constexpr int kAcMaxN = kNsMaxA + 1;
+
+struct AcParams {
+    const float *h, *h_boot, *w, *b;
+    const int64_t* actions;
+    const double* rewards;
+    const uint8_t* game_overs;
+    const int32_t *seg_off, *seg_len;
+    int S, rows, mode, huber, K, A;
+    double discount, gae_lambda;
+    float beta_entropy, v_weight, p_weight;
+    float *z, *dz, *probs, *targets, *advantages, *bootstrap, *dh;
+    uint16_t* dh_planes;
+    int64_t dh_plane_stride;
+    float* workspace;
+};
+
+// p = softmax(z[1..A]) in fp32: exp(x - max) / sum, the sum in index order.  cb200_categorical_act uses the same code, so
+// acting and learning see the same probabilities.
+__device__ __forceinline__ void ac_softmax(const float (&z)[kAcMaxN], int A, float (&p)[kNsMaxA]) {
+    float m = z[1];
+#pragma unroll
+    for (int a = 1; a < kNsMaxA; ++a)
+        if (a < A) m = fmaxf(m, z[a + 1]);
+    float s = 0.f;
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a) {
+        p[a] = a < A ? expf(z[a + 1] - m) : 0.f;
+        s += p[a];
+    }
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a) p[a] = p[a] / s;
+}
+
+// first-order scipy.signal.lfilter([1], [1, -c]) step, as its C loop evaluates it: y = z + 1 * x, then the delay
+// z' = x * 0 - y * (-c)
+__device__ __forceinline__ double ac_lfilter(double x, double& z, double c) {
+    const double y = __dadd_rn(z, x);
+    z = __dsub_rn(__dmul_rn(x, 0.0), __dmul_rn(y, -c));
+    return y;
+}
+
+template <int KPL>
+__global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcParams p) {
+    // Wt [N][K] | per warp: row buffer [K] | dW [N][K] | db [32]
+    extern __shared__ __align__(16) float ac_smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int gw = blockIdx.x * kNsWarps + warp, nwarps = gridDim.x * kNsWarps;
+    const int A = p.A, K = p.K, N = p.A + 1;
+    float* wt = ac_smem;
+    float* rowbuf = ac_smem + N * K + warp * (K + N * K + 32);
+    float* dwacc = rowbuf + K;
+    float* dbacc = dwacc + N * K;
+    for (int i = threadIdx.x; i < N * K; i += blockDim.x) {               // W [K, N] row-major -> Wt [N][K]
+        const int k = i / N, n = i - k * N;
+        wt[n * K + k] = __ldg(p.w + i);
+    }
+    for (int i = lane; i < N * K + 32; i += 32) dwacc[i] = 0.f;
+    int nseg = 0, used = 0;
+    for (int s = lane; s < p.S; s += 32) {
+        const int L = p.seg_len[s];
+        if (L > 0) {
+            nseg += 1;
+            used += L;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        nseg += __shfl_xor_sync(0xffffffffu, nseg, o);
+        used += __shfl_xor_sync(0xffffffffu, used, o);
+    }
+    __syncthreads();
+    const float w = nseg > 0 ? 1.0f / (float)nseg : 0.f;                 // the mean over segments
+    const float eps = 1.1920928955078125e-07f;                            // np.finfo(np.float32).eps
+    float acc_loss = 0.f;
+    if (gw < p.S) {
+        const int s = gw, L = p.seg_len[s], o = p.seg_off[s];
+        const bool valid = L > 0 && o >= 0 && (int64_t)o + L <= p.rows;
+        const bool terminal = valid && p.game_overs[o + L - 1];
+        float hv[KPL], z[kAcMaxN];
+        float vnext = 0.f;                                                // V(s'_last), 0 after a terminal state
+        if (valid && !terminal) {
+            ns_dot<KPL, kAcMaxN>(p.h_boot + (size_t)s * K, wt, p.b, 1, K, lane, hv, z);
+            vnext = z[0];
+        }
+        if (p.bootstrap && lane == 0) p.bootstrap[s] = vnext;
+        const double gamma = p.discount, gl = __dmul_rn(p.discount, p.gae_lambda);
+        const float gamma32 = (float)p.discount;
+        // A_VALUE: R; GAE: the advantage filter's delay za and the discounted-return filter's delay zr, started on
+        // values[-1] (= vnext)
+        double R = 0.0, za = 0.0, zr = 0.0;
+        bool boot_pending = !terminal;
+        if (p.mode != CB200_AC_A_VALUE) ac_lfilter((double)vnext, zr, gamma);
+        const float inv_l = valid ? 1.0f / (float)L : 0.f;
+        const float c = w * inv_l;
+        float seg_sum = 0.f;
+        for (int i = (valid ? L : 0) - 1; i >= 0; --i) {
+            const int r = o + i;
+            const double rw = p.rewards[r];
+            ns_dot<KPL, kAcMaxN>(p.h + (size_t)r * K, wt, p.b, N, K, lane, hv, z);     // hv = this row's features
+            const float v = z[0];
+            double target, adv;
+            if (p.mode == CB200_AC_A_VALUE) {
+                // R = r_i + discount * R; right after a bootstrap, python float * np.float32 is an fp32 product
+                R = boot_pending ? __dadd_rn(rw, (double)__fmul_rn(gamma32, vnext)) : __dadd_rn(rw, __dmul_rn(gamma, R));
+                boot_pending = false;
+                target = R;
+                adv = __dsub_rn(R, (double)v);
+            } else {
+                // deltas = rewards + discount * values[1:] - values[:-1]: every discount * value is an fp32 product
+                const double delta = __dsub_rn(__dadd_rn(rw, (double)__fmul_rn(gamma32, vnext)), (double)v);
+                adv = ac_lfilter(delta, za, gl);
+                const double ret = ac_lfilter(rw, zr, gamma);
+                target = p.mode == CB200_AC_GAE_VALUE ? __dadd_rn(adv, (double)v) : ret;
+            }
+            vnext = v;
+            const float t32 = (float)target, a32 = (float)adv;
+            // policy: p = softmax(logits); Categorical(probs = p + eps): log_softmax(log(p + eps)), probs not renormalised
+            float pr[kNsMaxA], ls[kNsMaxA];
+            ac_softmax(z, A, pr);
+            float su = 0.f;
+#pragma unroll
+            for (int a = 0; a < kNsMaxA; ++a)
+                if (a < A) su += pr[a] + eps;
+            const float lse = logf(su);
+            float ent = 0.f;
+#pragma unroll
+            for (int a = 0; a < kNsMaxA; ++a)
+                if (a < A) {
+                    ls[a] = logf(pr[a] + eps) - lse;
+                    ent = fmaf(-(pr[a] + eps), ls[a], ent);
+                }
+            const int64_t act = p.actions[r];
+            const bool in_range = act >= 0 && act < A;
+            float logp = 0.f, u_act = 1.f;
+#pragma unroll
+            for (int a = 0; a < kNsMaxA; ++a)
+                if (a == act) {
+                    logp = ls[a];
+                    u_act = pr[a] + eps;
+                }
+            // loss terms of this row: VHead (weight v_weight), -log pi(a) A (weight p_weight), -beta H
+            const float e = v - t32;
+            float lv, gv;
+            if (p.huber) {
+                const float ae = fabsf(e);
+                const float qq = fminf(ae, 1.0f);
+                lv = 0.5f * qq * qq + (ae - qq);
+                gv = fmaxf(-1.0f, fminf(e, 1.0f));
+            } else {
+                lv = e * e;
+                gv = 2.0f * e;
+            }
+            const float lp = in_range ? -p.p_weight * logp * a32 : 0.f;
+            seg_sum += p.v_weight * lv + lp - p.beta_entropy * ent;
+            // dL/dZ: d/du_k = c (-p_weight A ([k = a] / u_a - 1 / su) + beta ls_k) with u = p + eps, then the softmax
+            // Jacobian dz_k = p_k (g_k - sum_j p_j g_j)
+            const float cp = in_range ? -c * p.p_weight * a32 : 0.f, cb = c * p.beta_entropy, inv_su = 1.0f / su;
+            float g[kNsMaxA], pg = 0.f;
+#pragma unroll
+            for (int a = 0; a < kNsMaxA; ++a)
+                if (a < A) {
+                    g[a] = fmaf(cb, ls[a], cp * ((a == act ? 1.0f / u_act : 0.f) - inv_su));
+                    pg = fmaf(pr[a], g[a], pg);
+                }
+            float dz[kAcMaxN];
+            dz[0] = c * p.v_weight * gv;
+#pragma unroll
+            for (int a = 0; a < kNsMaxA; ++a) dz[a + 1] = a < A ? pr[a] * (g[a] - pg) : 0.f;
+            if (lane == 0) {
+#pragma unroll
+                for (int n = 0; n < kAcMaxN; ++n)
+                    if (n < N) {
+                        p.z[(size_t)r * N + n] = z[n];
+                        if (p.dz) p.dz[(size_t)r * N + n] = dz[n];
+                    }
+                if (p.probs) {
+#pragma unroll
+                    for (int a = 0; a < kNsMaxA; ++a)
+                        if (a < A) p.probs[(size_t)r * A + a] = pr[a];
+                }
+                if (p.targets) p.targets[r] = t32;
+                if (p.advantages) p.advantages[r] = a32;
+#pragma unroll
+                for (int n = 0; n < kAcMaxN; ++n)
+                    if (n < N) dbacc[n] += dz[n];
+            }
+            __syncwarp();                                                   // the previous row's readers are done
+#pragma unroll
+            for (int j = 0; j < KPL; ++j) {
+                const int k = lane + 32 * j;
+                float sdh = 0.f;
+#pragma unroll
+                for (int n = 0; n < kAcMaxN; ++n)
+                    if (n < N) {
+                        sdh = fmaf(dz[n], wt[n * K + k], sdh);
+                        dwacc[n * K + k] = fmaf(hv[j], dz[n], dwacc[n * K + k]);
+                    }
+                rowbuf[k] = hv[j] > 0.f ? sdh : 0.f;                        // relu'(h) on the post-activation value
+            }
+            __syncwarp();
+            head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+        }
+        acc_loss = __fmul_rn(__fmul_rn(seg_sum, inv_l), w);
+    }
+    // padding rows [used, rows): zero outputs and dh
+    for (int r = used + gw; r < p.rows; r += nwarps) {
+        __syncwarp();
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) rowbuf[lane + 32 * j] = 0.f;
+        for (int n = lane; n < N; n += 32) {
+            p.z[(size_t)r * N + n] = 0.f;
+            if (p.dz) p.dz[(size_t)r * N + n] = 0.f;
+            if (p.probs && n < A) p.probs[(size_t)r * A + n] = 0.f;
+        }
+        if (lane == 0) {
+            if (p.targets) p.targets[r] = 0.f;
+            if (p.advantages) p.advantages[r] = 0.f;
+        }
+        __syncwarp();
+        head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+    }
+    __syncwarp();
+    // per-warp partials in dqn_head_reduce_kernel's layout: [dW (K * N) | db (N) | loss (1)]
+    float* part = p.workspace + (size_t)gw * ((size_t)K * N + N + 1);
+#pragma unroll
+    for (int j = 0; j < KPL; ++j)
+        for (int n = 0; n < N; ++n) part[((size_t)lane + 32 * j) * N + n] = dwacc[n * K + lane + 32 * j];
+    if (lane == 0) {
+        for (int n = 0; n < N; ++n) part[(size_t)K * N + n] = dbacc[n];
+        part[(size_t)K * N + N] = acc_loss;
+    }
+}
+
+// one thread per environment: p = softmax of the policy logits (columns 1..A of z), then np.random.choice's
+// inverse-cdf draw (cdf = cumsum(float64(p)), cdf /= cdf[-1], the number of entries <= u) or the first argmax
+__global__ void categorical_act_kernel(const float* __restrict__ z, int64_t envs, int A, const double* __restrict__ u,
+                                       int64_t* __restrict__ actions, float* __restrict__ probs) {
+    const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= envs) return;
+    float zz[kAcMaxN], pr[kNsMaxA];
+#pragma unroll
+    for (int n = 0; n < kAcMaxN; ++n) zz[n] = n <= A ? z[e * (A + 1) + n] : 0.f;
+    ac_softmax(zz, A, pr);
+    int pick = 0;
+    if (u) {
+        double cdf[kNsMaxA], c = 0.0;
+#pragma unroll
+        for (int a = 0; a < kNsMaxA; ++a)
+            if (a < A) {
+                c = __dadd_rn(c, (double)pr[a]);
+                cdf[a] = c;
+            }
+        const double x = u[e];
+#pragma unroll
+        for (int a = 0; a < kNsMaxA; ++a)
+            if (a < A) pick += __ddiv_rn(cdf[a], c) <= x ? 1 : 0;
+        pick = min(pick, A - 1);
+    } else {
+        float m = pr[0];
+#pragma unroll
+        for (int a = 1; a < kNsMaxA; ++a)
+            if (a < A && (pr[a] > m || (pr[a] != pr[a] && m == m))) {     // np.argmax: the first maximum (or NaN)
+                m = pr[a];
+                pick = a;
+            }
+    }
+    actions[e] = pick;
+    if (probs) {
+#pragma unroll
+        for (int a = 0; a < kNsMaxA; ++a)
+            if (a < A) probs[e * A + a] = pr[a];
     }
 }
 
@@ -1259,6 +1541,73 @@ int cb200_polyak(float* target, const float* online, int64_t n, double rate, voi
     CB200_CHECK_ARG(target && online && n > 0, "bad arguments");
     CB200_LAUNCH(polyak_kernel, flat_grid(n), 256, 0, as_stream(stream), target, online, n, (float)rate,
                  (float)(1.0 - rate));
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_actor_critic_head(const cb200_actor_critic_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->mode >= CB200_AC_A_VALUE && d->mode <= CB200_AC_GAE_VALUE, "unknown mode");
+    CB200_CHECK_ARG(d->h && d->h_boot && d->w && d->b && d->actions && d->rewards && d->game_overs && d->seg_offsets &&
+                        d->seg_lengths && d->z && d->dw && d->db && d->workspace,
+                    "null pointer");
+    CB200_CHECK_ARG(d->segments >= 1 && d->segments <= (1 << 20), "1 <= segments <= 2^20");
+    CB200_CHECK_ARG(d->rows >= 1 && d->rows <= (1 << 24), "1 <= rows <= 2^24");
+    CB200_CHECK_ARG(d->n_actions >= 1 && d->n_actions <= kNsMaxA, "1 <= n_actions <= 18");
+    CB200_CHECK_ARG(d->features == 256 || d->features == 512, "features must be 256 or 512");
+    CB200_CHECK_ARG(!d->dh_planes || (d->dh_plane_stride % 8 == 0 && d->rows % 8 == 0), "planes: rows % 8, stride % 8");
+    AcParams p;
+    p.h = d->h; p.h_boot = d->h_boot; p.w = d->w; p.b = d->b;
+    p.actions = d->actions; p.rewards = d->rewards; p.game_overs = d->game_overs;
+    p.seg_off = d->seg_offsets; p.seg_len = d->seg_lengths;
+    p.S = d->segments; p.rows = (int)d->rows; p.mode = d->mode; p.huber = d->huber;
+    p.K = d->features; p.A = d->n_actions; p.discount = d->discount; p.gae_lambda = d->gae_lambda;
+    p.beta_entropy = d->beta_entropy; p.v_weight = d->v_weight; p.p_weight = d->p_weight;
+    p.z = d->z; p.dz = d->dz; p.probs = d->probs; p.targets = d->targets; p.advantages = d->advantages;
+    p.bootstrap = d->bootstrap; p.dh = d->dh;
+    p.dh_planes = static_cast<uint16_t*>(d->dh_planes); p.dh_plane_stride = d->dh_plane_stride;
+    p.workspace = d->workspace;
+    const unsigned grid = (unsigned)((p.S + kNsWarps - 1) / kNsWarps);
+    const int nparts = (int)grid * kNsWarps;                   // idle warps write zero partials
+    const int N = p.A + 1;
+    cudaStream_t st = as_stream(stream);
+    // up to 203 KB at K = 512, 1 + A = 19 (the staged kernel and four warps' dW slices): opted into once per
+    // instantiation and device, at the size of the largest shape
+    auto smem_of = [](int N, int K) { return (size_t)(N * K + kNsWarps * (K + N * K + 32)) * sizeof(float); };
+    const size_t smem = smem_of(N, p.K);
+    static bool attr_set[kMaxDevices][2] = {};
+    int dev = 0;
+    CB200_CUDA(cudaGetDevice(&dev));
+    CB200_CHECK_ARG(dev < kMaxDevices, "device ordinal out of range");
+    const int ti = p.K == 512 ? 1 : 0;
+    if (!attr_set[dev][ti]) {
+        if (ti)
+            CB200_CUDA(cudaFuncSetAttribute(actor_critic_head_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem_of(kAcMaxN, 512)));
+        else
+            CB200_CUDA(cudaFuncSetAttribute(actor_critic_head_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem_of(kAcMaxN, 256)));
+        attr_set[dev][ti] = true;
+    }
+    if (p.K == 512) {
+        CB200_LAUNCH(actor_critic_head_kernel<16>, grid, 32 * kNsWarps, smem, st, p);
+    } else {
+        CB200_LAUNCH(actor_critic_head_kernel<8>, grid, 32 * kNsWarps, smem, st, p);
+    }
+    const int n_out = p.K * N + N + 1;
+    CB200_LAUNCH(dqn_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, p.workspace, nparts, n_out,
+                 p.K * N, N, 1.0f, d->dw, d->db, d->loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_categorical_act(const float* z, int64_t envs, int32_t n_actions, const double* uniforms, int64_t* actions,
+                          float* probs, void* stream) {
+    CB200_CHECK_ARG(z && actions, "null pointer");
+    CB200_CHECK_ARG(envs >= 1 && envs <= (1 << 24), "1 <= envs <= 2^24");
+    CB200_CHECK_ARG(n_actions >= 1 && n_actions <= kNsMaxA, "1 <= n_actions <= 18");
+    CB200_LAUNCH(categorical_act_kernel, (unsigned)((envs + 127) / 128), 128, 0, as_stream(stream), z, envs, n_actions,
+                 uniforms, actions, probs);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

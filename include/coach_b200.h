@@ -533,6 +533,73 @@ typedef struct cb200_nstep_q_head_desc {
 
 int cb200_nstep_q_head(const cb200_nstep_q_head_desc* n_desc, void* stream);
 
+/* Fused actor-critic head (agents/actor_critic_agent.py:111-165, heads/v_head.py, heads/policy_head.py): ONE
+ * Dense(1 + n_actions) on one feature layer, column 0 the VHead V, columns 1..n_actions the PolicyHead logits, trained
+ * on the segment table of cb200_nstep_q_head (slot s covers rows [seg_offsets[s], + seg_lengths[s]), length 0 = unused;
+ * rows [n, rows) are padding and get zero outputs and dh).  Per segment of length L, with B = V(h_boot[s]) (0 when the
+ * segment's last game_over is set) and gl = discount * gae_lambda (fp64), walking i = L-1 .. 0, all in fp64 with _rn:
+ *   A_VALUE     R = r_i + discount R from R = B; the first step after a bootstrap is numpy's python float *
+ *               np.float32: (float)discount * B rounded in fp32, then added to r_i.  target R, advantage R - V_i.
+ *   GAE         delta_i = (r_i + fp32((float)discount * V_{i+1})) - V_i with V_L = B; advantage = the
+ *               scipy.signal.lfilter([1], [1, -gl]) recurrence A_i = delta_i + gl A_{i+1}; target = the lfilter
+ *               discounted sum of [r_0 .. r_{L-1}, B] with discount (GAE), or A_i + V_i (GAE_VALUE:
+ *               estimate_state_value_using_gae).
+ *   target and advantage are rounded to fp32.  p = softmax(logits) (fp32); u = p + FLT_EPSILON; ls = log u - log sum u;
+ *   H = -sum_k u_k ls_k (tf Categorical(probs = p + eps), probs not renormalised).
+ *   loss = (1/S) sum_s (1/L) sum_i [v_weight l(V_i - target_i) - p_weight ls_{a_i} A_i - beta_entropy H_i],
+ *   l = squared error or Huber (delta 1); a row whose action is outside [0, n_actions) has no policy term.
+ *   dz = dL/dZ over all 1 + n_actions columns, dW = h^T dz, db = sum_i dz_i, dh = (dz W^T) relu'(h).
+ * features 256 or 512, n_actions <= 18.  Deterministic: per-warp partials reduced in a fixed order by a second launch,
+ * no atomics; repeat calls and graph replays give the same bits. */
+typedef struct cb200_actor_critic_head_desc {
+    const float* h;             /* [rows, features] post-ReLU features of s                                               */
+    const float* h_boot;        /* [segments, features] features of each segment's last s' (online network)             */
+    const float* w;             /* head kernel [features, 1 + n_actions] and bias [1 + n_actions]                        */
+    const float* b;
+    const int64_t* actions;     /* [rows]                                                                                 */
+    const double* rewards;      /* [rows]                                                                                 */
+    const uint8_t* game_overs;  /* [rows]                                                                                 */
+    const int32_t* seg_offsets; /* [segments]                                                                             */
+    const int32_t* seg_lengths; /* [segments], 0 = unused slot                                                           */
+    int32_t segments;           /* slots in the table, 1 .. 2^20                                                         */
+    int64_t rows;               /* rows of the feature / output buffers, 1 .. 2^24                                       */
+    double discount;
+    double gae_lambda;
+    int32_t mode;               /* CB200_AC_*                                                                             */
+    int32_t huber;              /* VHead loss: 1 tf.losses.huber_loss(delta 1), 0 squared error                           */
+    float beta_entropy;
+    float v_weight;             /* VHead loss weight (0.5)                                                                */
+    float p_weight;             /* PolicyHead loss weight (1.0)                                                           */
+    int32_t features;           /* 256 or 512                                                                             */
+    int32_t n_actions;          /* 1 .. 18                                                                                */
+    float* z;                   /* out [rows, 1 + n_actions]: V | logits                                                  */
+    float* dz;                  /* out, optional [rows, 1 + n_actions]: dL/dZ                                             */
+    float* loss;                /* out scalar, optional                                                                   */
+    float* probs;               /* out, optional [rows, n_actions]                                                        */
+    float* targets;             /* out, optional [rows]: V targets (fp32)                                                 */
+    float* advantages;          /* out, optional [rows] (fp32)                                                            */
+    float* bootstrap;           /* out, optional [segments]: B                                                            */
+    float* dh;                  /* out, optional: [rows, features] dL/d(pre-activation of the feature layer)             */
+    void* dh_planes;            /* out, optional: the same as tiled bf16 hi / mid / lo planes                             */
+    int64_t dh_plane_stride;
+    float* dw;                  /* out [features, 1 + n_actions]                                                          */
+    float* db;                  /* out [1 + n_actions]                                                                    */
+    float* workspace;           /* ceil(segments / 4) * 4 * (features * (1 + n_actions) + n_actions + 2) floats          */
+} cb200_actor_critic_head_desc;
+
+#define CB200_AC_A_VALUE 0
+#define CB200_AC_GAE 1
+#define CB200_AC_GAE_VALUE 2
+
+int cb200_actor_critic_head(const cb200_actor_critic_head_desc* ac_desc, void* stream);
+
+/* Categorical acting (exploration_policies/categorical.py:36-47): z [envs, 1 + n_actions] as the actor-critic head
+ * lays it out (V | logits); p = softmax(logits) with the head's code.  uniforms [envs] (np.random.random_sample):
+ * np.random.choice's draw, cdf = cumsum(double(p)) in index order, cdf /= cdf[-1], action = the number of entries
+ * <= u; uniforms NULL: the first argmax (evaluation).  actions [envs] out, probs [envs, n_actions] out, optional. */
+int cb200_categorical_act(const float* z, int64_t envs, int32_t n_actions, const double* uniforms, int64_t* actions,
+                          float* probs, void* stream);
+
 /* Acting values of an ensemble, q [envs, heads * n_actions] -> out [envs, n_actions], in the exploration policies' fp32
  * numpy arithmetic (exploration_policies/bootstrapped.py:70-84, ucb.py:70-83):
  *   SELECT  the row of head[e] (Bootstrapped, training)
