@@ -571,10 +571,17 @@ __device__ __forceinline__ void bulk_pipeline(const GatherParams& gp, int64_t lo
         fence_proxy_async_smem();
         bulk_s2g(dst, stage_mem + (size_t)st * gp.stage_bytes, bytes);
         bulk_commit();
-        // refill the stage whose store was issued one iteration ago (its smem read has had time to drain)
-        if (k >= 1 && (k - 1 + S) < cnt) {
-            bulk_wait_read<1>();
-            issue_load(k - 1 + S);
+        // refill the stage whose store was issued one iteration ago (its smem read has had time to drain).  With one
+        // stage that stage is this iteration's: its store must finish reading now, and the load of item k + 1 must be
+        // in flight before the next wait, or that wait never completes.
+        if (S > 1) {
+            if (k >= 1 && (k - 1 + S) < cnt) {
+                bulk_wait_read<1>();
+                issue_load(k - 1 + S);
+            }
+        } else if (k + 1 < cnt) {
+            bulk_wait_read<0>();
+            issue_load(k + 1);
         }
     }
     bulk_wait_all<0>();
@@ -1117,7 +1124,7 @@ int cb200_host_priorities(const double* h_err, int64_t n, double epsilon, double
                           double* h_p_raw) {
     CB200_CHECK_ARG(n >= 0 && (n == 0 || (h_err && h_p_alpha && h_p_raw)), "bad arguments");
     for (int64_t i = 0; i < n; ++i)
-        if (h_err[i] < 0) {
+        if (!(h_err[i] >= 0)) {   // negative or NaN, as cb200_per_priorities_device
             set_error("cb200_host_priorities: The priorities must be non-negative values");
             return CB200_ERR_INVALID_ARGUMENT;
         }

@@ -91,7 +91,7 @@ int cb200_per_priorities_device(const double* err, int64_t n, double epsilon, do
 
 /* Same arithmetic with the host's libm `pow` -- bit-identical to the reference on the same machine.  Synchronous,
  * HOST pointers; the agent overlaps it with the network backward pass.  Returns CB200_ERR_INVALID_ARGUMENT (and
- * processes nothing) if an error value is negative. */
+ * processes nothing) if an error value is negative or NaN. */
 int cb200_host_priorities(const double* h_err, int64_t n, double epsilon, double alpha, double* h_p_alpha,
                           double* h_p_raw);
 
