@@ -179,7 +179,8 @@ __global__ void __launch_bounds__(256) axpby_2d_kernel(const float* __restrict__
 
 // DDPG / TD3 / SAC bootstrapped targets, evaluated like the numpy expression (fp64 rewards, fp32 network output):
 //   y = r + (1 - done) * discount * q_next      [done ignored when use_non_zero_discount_for_terminal_states]
-//   optional clip (ddpg_agent.py:163-164); written as fp32 (the TF placeholder dtype)
+//   optional clip (ddpg_agent.py:163-164) with np.clip's rules (NaN passes through, a value equal to a bound is kept);
+//   written as fp32 (the TF placeholder dtype)
 __global__ void __launch_bounds__(256) ac_td_targets_kernel(const double* __restrict__ rewards,
                                                             const uint8_t* __restrict__ dones,
                                                             const float* __restrict__ q_next, int ld_q, int64_t B,
@@ -197,15 +198,16 @@ __global__ void __launch_bounds__(256) ac_td_targets_kernel(const double* __rest
         const double nd = __dsub_rn(1.0, dones[i] ? 1.0 : 0.0);
         y = __dadd_rn(rewards[i], __dmul_rn(__dmul_rn(nd, discount), (double)q_next[i * ld_q]));
     }
-    if (use_clip) y = fmin(fmax(y, clip_lo), clip_hi);
+    if (use_clip) y = y < clip_lo ? clip_lo : (y > clip_hi ? clip_hi : y);
     out[i] = (float)y;
 }
 
-// out[i] = min(a[i], b[i])  (TD3 / SAC clipped double-Q)
+// out[i] = min(a[i], b[i])  (TD3 / SAC clipped double-Q) as tf.minimum evaluates it (std::min): `a` unless b < a, so
+// a tie of +0 and -0 keeps a's sign and a NaN in `a` passes through
 __global__ void __launch_bounds__(256) min2_kernel(const float* __restrict__ a, const float* __restrict__ b, int64_t n,
                                                    float* __restrict__ out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = fminf(a[i], b[i]);
+    if (i < n) out[i] = b[i] < a[i] ? b[i] : a[i];
 }
 
 // TD3 target policy smoothing (td3_agent.py:162-164): a = clip(a + clip(noise, -c, c), lo, hi), in place.  The
@@ -215,8 +217,11 @@ __global__ void __launch_bounds__(256) td3_smooth_kernel(float* __restrict__ act
                                                          int64_t n, double noise_clip, double lo, double hi) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const double nz = fmin(fmax(noise[i], -noise_clip), noise_clip);
-    actions[i] = (float)fmin(fmax(__dadd_rn((double)actions[i], nz), lo), hi);
+    // np.clip: NaN passes through, a value equal to a bound is kept
+    const double x = noise[i];
+    const double nz = x < -noise_clip ? -noise_clip : (x > noise_clip ? noise_clip : x);
+    const double y = __dadd_rn((double)actions[i], nz);
+    actions[i] = (float)(y < lo ? lo : (y > hi ? hi : y));
 }
 
 // =====================================================================================================================
@@ -463,7 +468,7 @@ __global__ void __launch_bounds__(256) sac_min_seed_kernel(const float* __restri
     const float s = 1.0f / (float)B;
     if (d1) d1[i] = first ? s : 0.f;
     if (d2) d2[i] = first ? 0.f : s;
-    if (qmin) qmin[i] = first ? q1[i] : q2[i];
+    if (qmin) qmin[i] = q2[i] < q1[i] ? q2[i] : q1[i];      // the value as tf.minimum (std::min): q1 unless q2 < q1
 }
 
 // out[i] = a[i] - b[i]   (value targets = min Q - log pi, soft_actor_critic_agent.py:244)

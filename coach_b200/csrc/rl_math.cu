@@ -179,7 +179,9 @@ __global__ void __launch_bounds__(256) stats_push_kernel(const float* __restrict
         sumsq[c] += r2[0];
     }
 }
-// mean = sum / count; std = sqrt(max((sumsq - count*mean^2) / max(count-1, 1), eps))   (:136-140)
+// mean = sum / count; std = sqrt(max((sumsq - count*mean^2) / max(count-1, 1), eps))   (:136-140), each operation
+// rounded on its own like numpy's (explicit _rn: nvcc would otherwise fuse count*mean^2 into the subtraction), so the
+// result is bit-identical to the reference's given the same sum, sumsq and count
 __global__ void stats_finalize_kernel(const double* __restrict__ sum, const double* __restrict__ sumsq, double count,
                                       double epsilon, int64_t cols, double* __restrict__ mean,
                                       double* __restrict__ std_) {
@@ -187,10 +189,11 @@ __global__ void stats_finalize_kernel(const double* __restrict__ sum, const doub
     if (c >= cols) return;
     const double m = sum[c] / count;
     mean[c] = m;
-    const double var = (sumsq[c] - count * (m * m)) / fmax(count - 1.0, 1.0);
+    const double var = __dsub_rn(sumsq[c], __dmul_rn(count, __dmul_rn(m, m))) / fmax(count - 1.0, 1.0);
     std_[c] = sqrt(fmax(var, epsilon));
 }
-// clip((x - mean) / (std + 1e-15), lo, hi)  (:162-164), fp64 math, fp32 result (what the network is fed)
+// clip((x - mean) / (std + 1e-15), lo, hi)  (:162-164), fp64 math, fp32 result (what the network is fed).  The clip is
+// np.clip's: a NaN passes through (a NaN observation stays visible) and an operand equal to a bound is kept as is.
 __global__ void __launch_bounds__(256) stats_normalize_kernel(const float* __restrict__ x, int64_t rows, int64_t cols,
                                                               const double* __restrict__ mean,
                                                               const double* __restrict__ std_, double lo, double hi,
@@ -199,7 +202,7 @@ __global__ void __launch_bounds__(256) stats_normalize_kernel(const float* __res
     if (i >= rows * cols) return;
     const int64_t c = i % cols;
     double v = ((double)x[i] - mean[c]) / (std_[c] + 1e-15);
-    v = fmin(fmax(v, lo), hi);
+    v = v < lo ? lo : (v > hi ? hi : v);
     if (out32) out32[i] = (float)v;
     if (out64) out64[i] = v;
 }

@@ -684,8 +684,10 @@ int cb200_axpby_2d(const float* src, int32_t ld_src, int64_t rows, int32_t cols,
                    int32_t ld_dst, void* stream);
 
 /* Bootstrapped critic targets of DDPG / TD3 / SAC (ddpg_agent.py:156-164, td3_agent.py:172-181,
- * soft_actor_critic_agent.py:265-266): y = r + (1 - done) * discount * q_next in fp64 (numpy), optional clip, stored
- * as fp32.  q_next is read with stride ld_q. */
+ * soft_actor_critic_agent.py:265-266): y = r + (1 - done) * discount * q_next in fp64 (numpy), optional clip (np.clip:
+ * a NaN passes through), stored as fp32; bit-exact with the numpy expression.  With
+ * use_non_zero_discount_for_terminal_states the product discount * q_next is fp32 (a Python float times a float32
+ * array).  q_next is read with stride ld_q. */
 int cb200_ac_td_targets(const double* rewards, const uint8_t* game_overs, const float* q_next, int32_t ld_q,
                         int64_t batch, double discount, int32_t use_non_zero_discount_for_terminal_states,
                         int32_t use_clip, double clip_lo, double clip_hi, float* targets_out, void* stream);
@@ -731,12 +733,14 @@ int cb200_naf_head(const cb200_naf_head_desc* desc, void* stream);
  * through, +-inf clips.  clip > 0. */
 int cb200_clip_by_value(float* g, int64_t n, float clip, void* stream);
 
-/* out = min(a, b) element-wise (clipped double-Q: td3_v_head.py:61, sac_q_head.py:84-86) */
+/* out = min(a, b) element-wise (clipped double-Q: td3_v_head.py:61, sac_q_head.py:84-86), as tf.minimum evaluates it:
+ * b where b < a, else a (a tie of +0 and -0 gives a; a NaN in a passes through, a NaN in b gives a) */
 int cb200_min2(const float* a, const float* b, int64_t n, float* out, void* stream);
 
 /* TD3 target policy smoothing (td3_agent.py:162-164): a = clip(a + clip(noise, -noise_clip, noise_clip), lo, hi);
  * noise is the fp64 np.random.normal draw, the sum and both clips are evaluated in fp64 like numpy does and rounded
- * to fp32 once (bit-exact with the reference, tests/golden/agent_prologues.npz) */
+ * to fp32 once (bit-exact with the reference, tests/golden/agent_prologues.npz).  Both clips are np.clip's: a NaN
+ * passes through and a value equal to a bound is kept. */
 int cb200_td3_smooth_actions(float* actions, const double* noise, int64_t n, double noise_clip, double lo, double hi,
                              void* stream);
 
@@ -822,7 +826,9 @@ int cb200_sac_policy_sample(const float* head_out, const float* eps, int64_t bat
 int cb200_sac_policy_grad(const float* head_out, const float* eps_logp, const float* eps_q, const float* dq_da,
                           int64_t batch, int32_t action_dim, float* d_head_out, void* stream);
 
-/* qmin = min(q1, q2) and the seeds d mean_b(qmin) / dq1, dq2 (sac_q_head.py:84-86); outputs may be NULL. */
+/* qmin = min(q1, q2) (the rule of cb200_min2) and the seeds d mean_b(qmin) / dq1, dq2 (sac_q_head.py:84-86): the
+ * seed float32(1) / float32(batch) goes to q1 where q1 <= q2 (tf.minimum's gradient rule), else to q2, and the other
+ * seed is 0.  Outputs may be NULL. */
 int cb200_sac_min_seed(const float* q1, const float* q2, int64_t batch, float* d1, float* d2, float* qmin,
                        void* stream);
 
@@ -860,8 +866,11 @@ int cb200_nstep_returns(const double* rewards, const int64_t* ep_start, const in
 /* NumpySharedRunningStats (utilities/shared_running_stats.py:115-164), used by ObservationNormalizationFilter
  * (filters/observation/observation_normalization_filter.py:71-78):
  *   push      : sum += sum_rows x, sumsq += sum_rows x^2   (fp64; the host adds `rows` to its count)
- *   finalize  : mean = sum/count; std = sqrt(max((sumsq - count*mean^2) / max(count-1, 1), epsilon))
- *   normalize : clip((x - mean) / (std + 1e-15), lo, hi) -> fp32 (network feed) and/or fp64 */
+ *   finalize  : mean = sum/count; std = sqrt(max((sumsq - count*mean^2) / max(count-1, 1), epsilon)), every
+ *               operation rounded on its own as numpy does (no fused multiply-add): bit-identical to the reference
+ *               given the same sum, sumsq and count.  count > 0.
+ *   normalize : clip((x - mean) / (std + 1e-15), lo, hi) -> fp32 (network feed) and/or fp64; bit-identical to numpy,
+ *               np.clip's rules (a NaN passes through).  At least one of out32 / out64 must be given. */
 int cb200_running_stats_push(const float* x, int64_t rows, int64_t cols, double* sum, double* sumsq, void* stream);
 int cb200_running_stats_finalize(const double* sum, const double* sumsq, double count, double epsilon, int64_t cols,
                                  double* mean, double* std_out, void* stream);
