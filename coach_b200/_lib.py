@@ -132,6 +132,21 @@ class ActorCriticHeadDesc(ctypes.Structure):
 AC_A_VALUE, AC_GAE, AC_GAE_VALUE = 0, 1, 2
 
 
+class PolicyGradientHeadDesc(ctypes.Structure):
+    """struct cb200_policy_gradient_head_desc"""
+    _fields_ = [("h", c_void_p), ("w", c_void_p), ("b", c_void_p), ("targets", c_void_p), ("actions", c_void_p),
+                ("cont_actions", c_void_p), ("max_abs_range", c_void_p), ("seg_offsets", c_void_p),
+                ("seg_lengths", c_void_p), ("segments", ctypes.c_int32), ("rows", c_i64),
+                ("continuous", ctypes.c_int32), ("features", ctypes.c_int32), ("n_outputs", ctypes.c_int32),
+                ("beta_entropy", c_float), ("z", c_void_p), ("policy", c_void_p), ("dz", c_void_p),
+                ("loss", c_void_p), ("dh", c_void_p), ("dh_planes", c_void_p), ("dh_plane_stride", c_i64),
+                ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p)]
+
+
+# cb200_pg_targets rescalers (the values of PolicyGradientRescaler)
+PG_TOTAL_RETURN, PG_FUTURE_RETURN, PG_NORMALIZED_BY_EPISODE, PG_NORMALIZED_BY_TIMESTEP = 0, 1, 2, 3
+
+
 # cb200_ensemble_action_values modes
 ENSEMBLE_SELECT, ENSEMBLE_UCB, ENSEMBLE_MEAN, ENSEMBLE_VOTE = 0, 1, 2, 3
 
@@ -189,6 +204,11 @@ PROTOTYPES = {
     "cb200_nstep_q_head": (c_int, [c_void_p, c_void_p]),
     "cb200_actor_critic_head": (c_int, [c_void_p, c_void_p]),
     "cb200_categorical_act": (c_int, [c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "cb200_pg_targets": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_int32, c_i64, ctypes.c_int32, c_void_p,
+                                 c_void_p, ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "cb200_policy_gradient_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_policy_act": (c_int, [c_void_p, c_i64, ctypes.c_int32, ctypes.c_int32, c_void_p, c_void_p, c_void_p,
+                                 c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "cb200_ensemble_action_values": (c_int, [c_void_p, c_i64, ctypes.c_int32, ctypes.c_int32, ctypes.c_int32, c_void_p,
                                              c_float, c_void_p, c_void_p]),
     "cb200_dueling_combine_fwd": (c_int, [c_void_p, c_void_p, c_i64, c_i64, c_void_p, c_void_p]),

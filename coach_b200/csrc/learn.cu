@@ -1027,6 +1027,54 @@ __device__ __forceinline__ double ac_lfilter(double x, double& z, double c) {
     return y;
 }
 
+// PolicyHead's discrete terms of one row (heads/policy_head.py:91-100), shared by the actor-critic and the policy
+// gradient heads: p = softmax(logits z[1..A]); Categorical(probs = p + eps): ls = log_softmax(log(p + eps)) (probs not
+// renormalised), H = -sum u ls, logp = ls[act] (0 for an action outside [0, A)), u_act = p[act] + eps, su = sum u.
+__device__ __forceinline__ void ac_policy_terms(const float (&z)[kAcMaxN], int A, int64_t act, float (&pr)[kNsMaxA],
+                                                float (&ls)[kNsMaxA], float& ent, float& logp, float& u_act,
+                                                float& su) {
+    const float eps = 1.1920928955078125e-07f;                            // np.finfo(np.float32).eps
+    ac_softmax(z, A, pr);
+    su = 0.f;
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a)
+        if (a < A) su += pr[a] + eps;
+    const float lse = logf(su);
+    ent = 0.f;
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a)
+        if (a < A) {
+            ls[a] = logf(pr[a] + eps) - lse;
+            ent = fmaf(-(pr[a] + eps), ls[a], ent);
+        }
+    logp = 0.f;
+    u_act = 1.f;
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a)
+        if (a == act) {
+            logp = ls[a];
+            u_act = pr[a] + eps;
+        }
+}
+// dL/d(logits) of -cp' logp(a) - cb' H per row, given cp = -(row weight) * (policy weight) * advantage (0 for an
+// action out of range) and cb = (row weight) * beta: d/du_k = cp ([k = a] / u_a - 1 / su) + cb ls_k with u = p + eps,
+// then the softmax Jacobian dz_k = p_k (g_k - sum_j p_j g_j); written to dz[off + k]
+template <int NOUT>
+__device__ __forceinline__ void ac_policy_dz(const float (&pr)[kNsMaxA], const float (&ls)[kNsMaxA], int A,
+                                             int64_t act, float u_act, float su, float cp, float cb, int off,
+                                             float (&dz)[NOUT]) {
+    const float inv_su = 1.0f / su;
+    float g[kNsMaxA], pg = 0.f;
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a)
+        if (a < A) {
+            g[a] = fmaf(cb, ls[a], cp * ((a == act ? 1.0f / u_act : 0.f) - inv_su));
+            pg = fmaf(pr[a], g[a], pg);
+        }
+#pragma unroll
+    for (int a = 0; a < kNsMaxA; ++a) dz[a + off] = a < A ? pr[a] * (g[a] - pg) : 0.f;
+}
+
 template <int KPL>
 __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcParams p) {
     // Wt [N][K] | per warp: row buffer [K] | dW [N][K] | db [32]
@@ -1058,7 +1106,6 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcP
     }
     __syncthreads();
     const float w = nseg > 0 ? 1.0f / (float)nseg : 0.f;                 // the mean over segments
-    const float eps = 1.1920928955078125e-07f;                            // np.finfo(np.float32).eps
     float acc_loss = 0.f;
     if (gw < p.S) {
         const int s = gw, L = p.seg_len[s], o = p.seg_off[s];
@@ -1103,29 +1150,10 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcP
             vnext = v;
             const float t32 = (float)target, a32 = (float)adv;
             // policy: p = softmax(logits); Categorical(probs = p + eps): log_softmax(log(p + eps)), probs not renormalised
-            float pr[kNsMaxA], ls[kNsMaxA];
-            ac_softmax(z, A, pr);
-            float su = 0.f;
-#pragma unroll
-            for (int a = 0; a < kNsMaxA; ++a)
-                if (a < A) su += pr[a] + eps;
-            const float lse = logf(su);
-            float ent = 0.f;
-#pragma unroll
-            for (int a = 0; a < kNsMaxA; ++a)
-                if (a < A) {
-                    ls[a] = logf(pr[a] + eps) - lse;
-                    ent = fmaf(-(pr[a] + eps), ls[a], ent);
-                }
+            float pr[kNsMaxA], ls[kNsMaxA], ent, logp, u_act, su;
             const int64_t act = p.actions[r];
             const bool in_range = act >= 0 && act < A;
-            float logp = 0.f, u_act = 1.f;
-#pragma unroll
-            for (int a = 0; a < kNsMaxA; ++a)
-                if (a == act) {
-                    logp = ls[a];
-                    u_act = pr[a] + eps;
-                }
+            ac_policy_terms(z, A, act, pr, ls, ent, logp, u_act, su);
             // loss terms of this row: VHead (weight v_weight), -log pi(a) A (weight p_weight), -beta H
             const float e = v - t32;
             float lv, gv;
@@ -1142,18 +1170,10 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcP
             seg_sum += p.v_weight * lv + lp - p.beta_entropy * ent;
             // dL/dZ: d/du_k = c (-p_weight A ([k = a] / u_a - 1 / su) + beta ls_k) with u = p + eps, then the softmax
             // Jacobian dz_k = p_k (g_k - sum_j p_j g_j)
-            const float cp = in_range ? -c * p.p_weight * a32 : 0.f, cb = c * p.beta_entropy, inv_su = 1.0f / su;
-            float g[kNsMaxA], pg = 0.f;
-#pragma unroll
-            for (int a = 0; a < kNsMaxA; ++a)
-                if (a < A) {
-                    g[a] = fmaf(cb, ls[a], cp * ((a == act ? 1.0f / u_act : 0.f) - inv_su));
-                    pg = fmaf(pr[a], g[a], pg);
-                }
+            const float cp = in_range ? -c * p.p_weight * a32 : 0.f, cb = c * p.beta_entropy;
             float dz[kAcMaxN];
             dz[0] = c * p.v_weight * gv;
-#pragma unroll
-            for (int a = 0; a < kNsMaxA; ++a) dz[a + 1] = a < A ? pr[a] * (g[a] - pg) : 0.f;
+            ac_policy_dz(pr, ls, A, act, u_act, su, cp, cb, 1, dz);
             if (lane == 0) {
 #pragma unroll
                 for (int n = 0; n < kAcMaxN; ++n)
@@ -1219,15 +1239,17 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcP
     }
 }
 
-// one thread per environment: p = softmax of the policy logits (columns 1..A of z), then np.random.choice's
-// inverse-cdf draw (cdf = cumsum(float64(p)), cdf /= cdf[-1], the number of entries <= u) or the first argmax
-__global__ void categorical_act_kernel(const float* __restrict__ z, int64_t envs, int A, const double* __restrict__ u,
-                                       int64_t* __restrict__ actions, float* __restrict__ probs) {
+// one thread per environment: p = softmax of the policy logits (row e of z: A columns from column `first`, row stride
+// ld), then np.random.choice's inverse-cdf draw (cdf = cumsum(float64(p)), cdf /= cdf[-1], the number of entries <= u)
+// or the first argmax.  The actor-critic layout is ld = 1 + A, first = 1; the policy gradient layout ld = A, first = 0.
+__global__ void categorical_act_kernel(const float* __restrict__ z, int ld, int first, int64_t envs, int A,
+                                       const double* __restrict__ u, int64_t* __restrict__ actions,
+                                       float* __restrict__ probs) {
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= envs) return;
     float zz[kAcMaxN], pr[kNsMaxA];
 #pragma unroll
-    for (int n = 0; n < kAcMaxN; ++n) zz[n] = n <= A ? z[e * (A + 1) + n] : 0.f;
+    for (int n = 0; n < kAcMaxN; ++n) zz[n] = (n >= 1 && n <= A) ? z[e * ld + first + n - 1] : 0.f;   // zz[0] unread
     ac_softmax(zz, A, pr);
     int pick = 0;
     if (u) {
@@ -1258,6 +1280,316 @@ __global__ void categorical_act_kernel(const float* __restrict__ z, int64_t envs
         for (int a = 0; a < kNsMaxA; ++a)
             if (a < A) probs[e * A + a] = pr[a];
     }
+}
+
+// ---- policy gradients (REINFORCE) ------------------------------------------------------------------------------------
+// Targets: the return-based rescalers of policy_gradients_agent.py:47-67 over whole episodes (one segment = one
+// episode), given the fp64 returns of cb200_nstep_returns; every fp64 operation is an explicit _rn intrinsic.
+
+// numpy's pairwise summation (np.add.reduce on a contiguous float64 array, loops_utils.h pairwise_sum) of f(i) for
+// i < n: below 8 terms a running sum; up to 128 terms eight accumulators over the blocks of 8, folded
+// ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7)), then the tail; above, the halves split at n/2 rounded down to a
+// multiple of 8.  The recursion runs on an explicit stack (at most 18 levels for n < 2^24).
+template <class F>
+__device__ double np_pairwise_sum(F f, int n) {
+    constexpr int kDepth = 20;
+    int lo[kDepth], len[kDepth], stage[kDepth];
+    double left[kDepth];
+    int sp = 0;
+    lo[0] = 0;
+    len[0] = n;
+    stage[0] = 0;
+    double r = 0.0;
+    for (;;) {
+        if (len[sp] > 128) {                                              // descend into the left half
+            int n2 = len[sp] / 2;
+            n2 -= n2 % 8;
+            stage[sp] = 1;
+            lo[sp + 1] = lo[sp];
+            len[sp + 1] = n2;
+            ++sp;
+            continue;
+        }
+        const int b = lo[sp], m = len[sp];
+        if (m < 8) {
+            r = -0.0;
+            for (int i = 0; i < m; ++i) r = __dadd_rn(r, f(b + i));
+        } else {
+            double acc[8];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) acc[j] = f(b + j);
+            int i = 8;
+            for (; i < m - (m % 8); i += 8)
+#pragma unroll
+                for (int j = 0; j < 8; ++j) acc[j] = __dadd_rn(acc[j], f(b + i + j));
+            r = __dadd_rn(__dadd_rn(__dadd_rn(acc[0], acc[1]), __dadd_rn(acc[2], acc[3])),
+                          __dadd_rn(__dadd_rn(acc[4], acc[5]), __dadd_rn(acc[6], acc[7])));
+            for (; i < m; ++i) r = __dadd_rn(r, f(b + i));
+        }
+        // return r to the parents: a left half starts the right half, a right half completes its parent
+        for (;;) {
+            if (sp == 0) return r;
+            --sp;
+            if (stage[sp] == 1) {
+                int n2 = len[sp] / 2;
+                n2 -= n2 % 8;
+                left[sp] = r;
+                stage[sp] = 2;
+                lo[sp + 1] = lo[sp] + n2;
+                len[sp + 1] = len[sp] - n2;
+                ++sp;
+                break;
+            }
+            r = __dadd_rn(left[sp], r);
+        }
+    }
+}
+
+// one block per segment slot: TOTAL_RETURN (R_0 on every row), FUTURE_RETURN (R) and NORMALIZED_BY_EPISODE
+// ((R - mean) / std with np.mean / np.std of the episode's returns, 0 when std == 0; policy_optimization_agent.py:62-71)
+__global__ void __launch_bounds__(256) pg_segment_targets_kernel(const double* __restrict__ ret,
+                                                                 const int32_t* __restrict__ seg_off,
+                                                                 const int32_t* __restrict__ seg_len, int64_t rows,
+                                                                 int mode, float* __restrict__ targets,
+                                                                 double* __restrict__ stats) {
+    __shared__ double mean_std[2];
+    const int s = blockIdx.x, L = seg_len[s], o = seg_off[s];
+    if (!(L > 0 && o >= 0 && (int64_t)o + L <= rows)) return;
+    const double* R = ret + o;
+    if (mode == CB200_PG_NORMALIZED_BY_EPISODE && threadIdx.x == 0) {
+        const double n = (double)L;
+        const double mean = __ddiv_rn(np_pairwise_sum([&](int i) { return R[i]; }, L), n);
+        const double var = __ddiv_rn(np_pairwise_sum([&](int i) {
+            const double x = __dsub_rn(R[i], mean);
+            return __dmul_rn(x, x);
+        }, L), n);
+        mean_std[0] = mean;
+        mean_std[1] = __dsqrt_rn(var);
+        if (stats) {
+            stats[2 * s] = mean;
+            stats[2 * s + 1] = mean_std[1];
+        }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < L; i += blockDim.x) {
+        double t;
+        if (mode == CB200_PG_TOTAL_RETURN) {
+            t = R[0];
+        } else if (mode == CB200_PG_FUTURE_RETURN) {
+            t = R[i];
+        } else {
+            const double sd = mean_std[1];
+            t = sd != 0.0 ? __ddiv_rn(__dsub_rn(R[i], mean_std[0]), sd) : 0.0;
+        }
+        targets[o + i] = (float)t;
+    }
+}
+
+// NORMALIZED_BY_TIMESTEP: one thread per timestep i, the segments folded in slot order into the running mean table
+// (update_episode_statistics, policy_optimization_agent.py:58-71: n_i += 1; m_i -= m_i / n_i; m_i += R_i / n_i), and
+// each row's baseline is the table right after its own segment's fold (learn_from_batch: R_i - m_i)
+__global__ void __launch_bounds__(256) pg_timestep_targets_kernel(const double* __restrict__ ret,
+                                                                  const int32_t* __restrict__ seg_off,
+                                                                  const int32_t* __restrict__ seg_len, int S,
+                                                                  int64_t rows, double* __restrict__ mean,
+                                                                  double* __restrict__ count, int table_len,
+                                                                  float* __restrict__ targets,
+                                                                  double* __restrict__ baselines) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rows) return;
+    const bool in_table = i < table_len;
+    double m = in_table ? mean[i] : 0.0, c = in_table ? count[i] : 0.0;
+    bool touched = false;
+    for (int s = 0; s < S; ++s) {
+        const int L = seg_len[s], o = seg_off[s];
+        if (!(L > 0 && o >= 0 && (int64_t)o + L <= rows) || i >= L) continue;
+        const int64_t r = o + i;
+        if (!in_table) {                                                  // longer than the table: no baseline
+            targets[r] = __int_as_float(0x7fc00000);
+            if (baselines) baselines[r] = __longlong_as_double(0x7ff8000000000000ll);
+            continue;
+        }
+        const double x = ret[r];
+        c = __dadd_rn(c, 1.0);
+        m = __dsub_rn(m, __ddiv_rn(m, c));
+        m = __dadd_rn(m, __ddiv_rn(x, c));
+        touched = true;
+        targets[r] = (float)__dsub_rn(x, m);
+        if (baselines) baselines[r] = m;
+    }
+    if (touched) {
+        mean[i] = m;
+        count[i] = c;
+    }
+}
+
+// Head: heads/policy_head.py:54-150 with policy_gradients_agent.py's loss, one Dense(N) on a feature layer.
+// Parallel over rows: a block owns kPgBlockRows consecutive rows, maps each to its segment slot in shared memory and
+// gives each warp kPgWarpRows of them; per row the xor-butterfly dot products of nstep_q_head_kernel, the row's loss,
+// dL/dZ (written out) and dL/dh.  pg_head_dw_kernel then forms dW = h^T dZ, db and the loss per 64-row chunk, and
+// dqn_head_reduce_kernel sums the chunks in a fixed order.
+constexpr int kPgWarps = 8;
+constexpr int kPgWarpRows = 8;
+constexpr int kPgBlockRows = kPgWarps * kPgWarpRows;
+constexpr int kPgChunk = 64;
+constexpr int kPgMaxD = 32;
+
+struct PgParams {
+    const float *h, *w, *b, *targets, *cont_actions, *range;
+    const int64_t* actions;
+    const int32_t *seg_off, *seg_len;
+    int S, rows, K, N, continuous;
+    float beta_entropy;
+    float *z, *policy, *dz, *rowloss, *dh;
+    uint16_t* dh_planes;
+    int64_t dh_plane_stride;
+};
+
+// the bounded Gaussian mean of the continuous head: tanh(z) * max_abs_range (policy_head.py:118-126); th = tanh(z)
+__device__ __forceinline__ float pg_mean(float z, float range, float& th) {
+    th = tanhf(z);
+    return th * range;
+}
+
+template <int KPL>
+__global__ void __launch_bounds__(32 * kPgWarps) pg_head_rows_kernel(PgParams p) {
+    // Wt [N][K] | row buffers [warps][K] | segment slot of each of the block's rows
+    extern __shared__ __align__(16) float pg_smem[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int N = p.N, K = p.K;
+    float* wt = pg_smem;
+    float* rowbuf = pg_smem + N * K + warp * K;
+    int* slot = reinterpret_cast<int*>(pg_smem + N * K + kPgWarps * K);
+    const int r0 = blockIdx.x * kPgBlockRows;
+    for (int i = threadIdx.x; i < N * K; i += blockDim.x) {               // W [K, N] row-major -> Wt [N][K]
+        const int k = i / N, n = i - k * N;
+        wt[n * K + k] = __ldg(p.w + i);
+    }
+    for (int j = threadIdx.x; j < kPgBlockRows; j += blockDim.x) slot[j] = -1;
+    __syncthreads();
+    for (int s = threadIdx.x; s < p.S; s += blockDim.x) {
+        const int L = p.seg_len[s], o = p.seg_off[s];
+        if (!(L > 0 && o >= 0 && (int64_t)o + L <= p.rows)) continue;
+        const int lo = max(o, r0), hi = min(o + L, r0 + kPgBlockRows);
+        for (int r = lo; r < hi; ++r) slot[r - r0] = s;
+    }
+    __syncthreads();
+    const float log2pi = 1.8378770664093453f;
+    for (int rr = 0; rr < kPgWarpRows; ++rr) {
+        const int r = r0 + warp * kPgWarpRows + rr;
+        if (r >= p.rows) break;
+        const int s = slot[r - r0];
+        float hv[KPL], z[kPgMaxD], dz[kPgMaxD], pol[kPgMaxD];
+        float row_loss = 0.f;
+#pragma unroll
+        for (int n = 0; n < kPgMaxD; ++n) z[n] = dz[n] = pol[n] = 0.f;
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) hv[j] = 0.f;
+        if (s >= 0) {
+            ns_dot<KPL, kPgMaxD>(p.h + (size_t)r * K, wt, p.b, N, K, lane, hv, z);
+            const float c = 1.0f / (float)p.seg_len[s];                   // the episode's mean
+            const float t = p.targets[r];
+            if (!p.continuous) {
+                // -mean(log pi(a) t) - beta mean(H) with Categorical(probs = softmax + eps)
+                float zz[kAcMaxN], pr[kNsMaxA], ls[kNsMaxA], ent, logp, u_act, su;
+                zz[0] = 0.f;
+#pragma unroll
+                for (int a = 0; a < kNsMaxA; ++a) zz[a + 1] = z[a];
+                const int64_t act = p.actions[r];
+                const bool in_range = act >= 0 && act < N;
+                ac_policy_terms(zz, N, act, pr, ls, ent, logp, u_act, su);
+                row_loss = c * ((in_range ? -logp * t : 0.f) - p.beta_entropy * ent);
+                ac_policy_dz(pr, ls, N, act, u_act, su, in_range ? -c * t : 0.f, c * p.beta_entropy, 0, dz);
+#pragma unroll
+                for (int a = 0; a < kNsMaxA; ++a) pol[a] = pr[a];
+            } else {
+                // MultivariateNormalDiag(mean, 1): log pi(x) = -|x - mean|^2 / 2 - D log(2 pi) / 2; its entropy
+                // D (1 + log(2 pi)) / 2 is a constant (the std is the all-ones policy_stdev variable)
+                float sq = 0.f;
+#pragma unroll
+                for (int d = 0; d < kPgMaxD; ++d)
+                    if (d < N) {
+                        const float rg = __ldg(p.range + d);
+                        float th;
+                        const float mu = pg_mean(z[d], rg, th);
+                        const float diff = p.cont_actions[(size_t)r * N + d] - mu;
+                        sq = fmaf(diff, diff, sq);
+                        pol[d] = mu;
+                        dz[d] = ((-c * t) * diff) * rg * (1.0f - th * th);
+                    }
+                const float logp = -0.5f * sq - 0.5f * (float)N * log2pi;
+                const float ent = 0.5f * (float)N * (1.0f + log2pi);
+                row_loss = c * (-logp * t - p.beta_entropy * ent);
+            }
+        }
+        if (lane == 0) {
+#pragma unroll
+            for (int n = 0; n < kPgMaxD; ++n)
+                if (n < N) {
+                    p.z[(size_t)r * N + n] = z[n];
+                    p.dz[(size_t)r * N + n] = dz[n];
+                    if (p.policy) p.policy[(size_t)r * N + n] = pol[n];
+                }
+            p.rowloss[r] = row_loss;
+        }
+        __syncwarp();                                                     // the previous row's readers are done
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) {
+            const int k = lane + 32 * j;
+            float sdh = 0.f;
+            if (s >= 0) {
+#pragma unroll
+                for (int n = 0; n < kPgMaxD; ++n)
+                    if (n < N) sdh = fmaf(dz[n], wt[n * K + k], sdh);
+            }
+            rowbuf[k] = (s >= 0 && hv[j] > 0.f) ? sdh : 0.f;              // relu'(h) on the post-activation value
+        }
+        __syncwarp();
+        head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+    }
+}
+
+// per 64-row chunk: dW[k, n] = sum_r h[r, k] dz[r, n], db[n] = sum_r dz[r, n] and the loss sum_r l_r, in row order,
+// into the chunk's partials [dW (K * N) | db (N) | loss (1)] (dqn_head_reduce_kernel's layout).  blockIdx.y strides over
+// the chunks (gridDim.y is at most 65535; 2^24 rows make 262144 chunks).
+__global__ void __launch_bounds__(256) pg_head_dw_kernel(const float* __restrict__ h, const float* __restrict__ dz,
+                                                         const float* __restrict__ rowloss, int rows, int K, int N,
+                                                         float* __restrict__ part) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const int KN = K * N, n_out = KN + N + 1;
+    if (i >= n_out) return;
+    const int chunks = (rows + kPgChunk - 1) / kPgChunk;
+    for (int ch = blockIdx.y; ch < chunks; ch += gridDim.y) {
+        const int r0 = ch * kPgChunk, r1 = min(rows, r0 + kPgChunk);
+        float s = 0.f;
+        if (i < KN) {
+            const int n = i / K, k = i - n * K;                           // a warp reads 32 consecutive features
+            for (int r = r0; r < r1; ++r) s = fmaf(__ldg(h + (size_t)r * K + k), __ldg(dz + (size_t)r * N + n), s);
+            part[(size_t)ch * n_out + (size_t)k * N + n] = s;
+            continue;
+        }
+        if (i < KN + N) {
+            for (int r = r0; r < r1; ++r) s += __ldg(dz + (size_t)r * N + (i - KN));
+        } else {
+            for (int r = r0; r < r1; ++r) s += __ldg(rowloss + r);
+        }
+        part[(size_t)ch * n_out + i] = s;
+    }
+}
+
+// acting of a continuous policy gradient head: thread per (environment, dimension); mean = tanh(z) * range (fp32),
+// then numpy's normal(loc = mean, scale) = loc + scale * z in fp64 on host standard normals (scale [envs, D]: each
+// environment's own noise), or the mean
+__global__ void pg_gaussian_act_kernel(const float* __restrict__ z, int64_t envs, int D, const float* __restrict__ range,
+                                       const double* __restrict__ normals, const double* __restrict__ scale,
+                                       double* __restrict__ actions, float* __restrict__ means) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= envs * D) return;
+    const int d = (int)(i % D);
+    float th;
+    const float mu = pg_mean(z[i], range[d], th);
+    actions[i] = normals ? __dadd_rn((double)mu, __dmul_rn(scale[i], normals[i])) : (double)mu;
+    if (means) means[i] = mu;
 }
 
 }  // namespace cb200
@@ -1606,8 +1938,112 @@ int cb200_categorical_act(const float* z, int64_t envs, int32_t n_actions, const
     CB200_CHECK_ARG(z && actions, "null pointer");
     CB200_CHECK_ARG(envs >= 1 && envs <= (1 << 24), "1 <= envs <= 2^24");
     CB200_CHECK_ARG(n_actions >= 1 && n_actions <= kNsMaxA, "1 <= n_actions <= 18");
-    CB200_LAUNCH(categorical_act_kernel, (unsigned)((envs + 127) / 128), 128, 0, as_stream(stream), z, envs, n_actions,
-                 uniforms, actions, probs);
+    CB200_LAUNCH(categorical_act_kernel, (unsigned)((envs + 127) / 128), 128, 0, as_stream(stream), z, n_actions + 1, 1,
+                 envs, n_actions, uniforms, actions, probs);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_pg_targets(const double* returns, const int32_t* seg_offsets, const int32_t* seg_lengths, int32_t segments,
+                     int64_t rows, int32_t rescaler, double* table_mean, double* table_count, int32_t table_len,
+                     float* targets, double* baselines, double* episode_stats, void* stream) {
+    CB200_CHECK_ARG(returns && seg_offsets && seg_lengths && targets, "null pointer");
+    CB200_CHECK_ARG(segments >= 1 && segments <= (1 << 20), "1 <= segments <= 2^20");
+    CB200_CHECK_ARG(rows >= 1 && rows <= (1 << 24), "1 <= rows <= 2^24");
+    CB200_CHECK_ARG(rescaler >= CB200_PG_TOTAL_RETURN && rescaler <= CB200_PG_NORMALIZED_BY_TIMESTEP,
+                    "unknown rescaler");
+    cudaStream_t st = as_stream(stream);
+    if (rescaler == CB200_PG_NORMALIZED_BY_TIMESTEP) {
+        CB200_CHECK_ARG(table_mean && table_count && table_len >= 1, "the timestep rescaler needs its table");
+        CB200_LAUNCH(pg_timestep_targets_kernel, (unsigned)((rows + 255) / 256), 256, 0, st, returns, seg_offsets,
+                     seg_lengths, segments, rows, table_mean, table_count, table_len, targets, baselines);
+    } else {
+        CB200_LAUNCH(pg_segment_targets_kernel, (unsigned)segments, 256, 0, st, returns, seg_offsets, seg_lengths, rows,
+                     rescaler, targets, episode_stats);
+    }
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_policy_gradient_head(const cb200_policy_gradient_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->h && d->w && d->b && d->targets && d->seg_offsets && d->seg_lengths && d->z && d->dw && d->db &&
+                        d->workspace && (d->continuous ? (d->cont_actions && d->max_abs_range) : d->actions != nullptr),
+                    "null pointer");
+    CB200_CHECK_ARG(d->segments >= 1 && d->segments <= (1 << 20), "1 <= segments <= 2^20");
+    CB200_CHECK_ARG(d->rows >= 1 && d->rows <= (1 << 24), "1 <= rows <= 2^24");
+    CB200_CHECK_ARG(d->continuous ? (d->n_outputs >= 1 && d->n_outputs <= kPgMaxD)
+                                  : (d->n_outputs >= 1 && d->n_outputs <= kNsMaxA),
+                    "1 <= n_outputs <= 18 (discrete) / 32 (continuous)");
+    CB200_CHECK_ARG(d->features == 256 || d->features == 512, "features must be 256 or 512");
+    CB200_CHECK_ARG(!d->dh_planes || (d->dh_plane_stride % 8 == 0 && d->rows % 8 == 0), "planes: rows % 8, stride % 8");
+    const int rows = (int)d->rows, K = d->features, N = d->n_outputs;
+    PgParams p;
+    p.h = d->h; p.w = d->w; p.b = d->b; p.targets = d->targets; p.cont_actions = d->cont_actions;
+    p.range = d->max_abs_range; p.actions = d->actions;
+    p.seg_off = d->seg_offsets; p.seg_len = d->seg_lengths;
+    p.S = d->segments; p.rows = rows; p.K = K; p.N = N; p.continuous = d->continuous ? 1 : 0;
+    p.beta_entropy = d->beta_entropy;
+    p.z = d->z; p.policy = d->policy; p.dh = d->dh;
+    p.dh_planes = static_cast<uint16_t*>(d->dh_planes); p.dh_plane_stride = d->dh_plane_stride;
+    // workspace: dL/dZ [rows, N] (unless given) | per-row losses [rows] | chunk partials
+    float* ws = d->workspace;
+    p.dz = d->dz ? d->dz : ws;
+    p.rowloss = ws + (size_t)rows * N;
+    float* part = p.rowloss + rows;
+    cudaStream_t st = as_stream(stream);
+    // up to 80 KB at K = 512, N = 32 (the staged kernel and eight row buffers): opted into once per instantiation and
+    // device, at the size of the largest shape
+    auto smem_of = [](int N, int K) {
+        return (size_t)(N * K + kPgWarps * K) * sizeof(float) + kPgBlockRows * sizeof(int);
+    };
+    static bool attr_set[kMaxDevices][2] = {};
+    int dev = 0;
+    CB200_CUDA(cudaGetDevice(&dev));
+    CB200_CHECK_ARG(dev < kMaxDevices, "device ordinal out of range");
+    const int ti = K == 512 ? 1 : 0;
+    if (!attr_set[dev][ti]) {
+        if (ti)
+            CB200_CUDA(cudaFuncSetAttribute(pg_head_rows_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem_of(kPgMaxD, 512)));
+        else
+            CB200_CUDA(cudaFuncSetAttribute(pg_head_rows_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                            (int)smem_of(kPgMaxD, 256)));
+        attr_set[dev][ti] = true;
+    }
+    const unsigned grid = (unsigned)((rows + kPgBlockRows - 1) / kPgBlockRows);
+    if (K == 512) {
+        CB200_LAUNCH(pg_head_rows_kernel<16>, grid, 32 * kPgWarps, smem_of(N, K), st, p);
+    } else {
+        CB200_LAUNCH(pg_head_rows_kernel<8>, grid, 32 * kPgWarps, smem_of(N, K), st, p);
+    }
+    const int n_out = K * N + N + 1, chunks = (rows + kPgChunk - 1) / kPgChunk;
+    const dim3 dw_grid((unsigned)((n_out + 255) / 256), (unsigned)min(chunks, 65535));
+    CB200_LAUNCH(pg_head_dw_kernel, dw_grid, 256, 0, st, d->h, p.dz, p.rowloss, rows, K, N, part);
+    CB200_LAUNCH(dqn_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, part, chunks, n_out, K * N, N, 1.0f,
+                 d->dw, d->db, d->loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_policy_act(const float* z, int64_t envs, int32_t n_outputs, int32_t continuous, const float* max_abs_range,
+                     const double* draws, const double* scale, int64_t* actions, float* probs, double* cont_actions,
+                     float* means, void* stream) {
+    CB200_CHECK_ARG(z != nullptr, "null pointer");
+    CB200_CHECK_ARG(envs >= 1 && envs <= (1 << 24), "1 <= envs <= 2^24");
+    cudaStream_t st = as_stream(stream);
+    if (!continuous) {
+        CB200_CHECK_ARG(actions != nullptr, "null pointer");
+        CB200_CHECK_ARG(n_outputs >= 1 && n_outputs <= kNsMaxA, "1 <= n_outputs <= 18");
+        CB200_LAUNCH(categorical_act_kernel, (unsigned)((envs + 127) / 128), 128, 0, st, z, n_outputs, 0, envs,
+                     n_outputs, draws, actions, probs);
+    } else {
+        CB200_CHECK_ARG(max_abs_range && cont_actions && (!draws || scale), "null pointer");
+        CB200_CHECK_ARG(n_outputs >= 1 && n_outputs <= kPgMaxD, "1 <= n_outputs <= 32");
+        const int64_t n = envs * n_outputs;
+        CB200_LAUNCH(pg_gaussian_act_kernel, (unsigned)((n + 127) / 128), 128, 0, st, z, envs, n_outputs, max_abs_range,
+                     draws, scale, cont_actions, means);
+    }
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

@@ -2,7 +2,7 @@
 
   rl_coach/agents/policy_optimization_agent.py:85-135    segment cut every t_max steps or at the episode's end
 
-shared by the agents that learn from such segments (N-step Q, A3C).  Each stream behaves like one asynchronous reference
+shared by the agents that learn from such segments (N-step Q, A3C, Policy Gradients).  Each stream behaves like one asynchronous reference
 worker: it has its own cut position and closes a segment when t_max (``num_steps_between_gradient_updates``) steps have
 passed since its last cut, or on game_over.  All segments closed at one lock-step are learned in ONE learn step.
 
@@ -27,7 +27,8 @@ def round32(n):
 
 
 class LockstepSegments(object):
-    def __init__(self, lib, device, observation_shape, num_envs, t_max):
+    def __init__(self, lib, device, observation_shape, num_envs, t_max, action_dim=None):
+        """action_dim: the action column holds float32 [action_dim] vectors (continuous actions) instead of int64"""
         self.lib = lib
         self.device = dev = torch.device(device)
         obs = tuple(observation_shape)
@@ -38,7 +39,8 @@ class LockstepSegments(object):
         obs_dtype = torch.uint8 if len(obs) == 3 else torch.float32
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)        # noqa: E731
         self.rollout = {"state": z((T * E,) + obs, obs_dtype), "next_state": z((T * E,) + obs, obs_dtype),
-                        "action": z(T * E, torch.int64), "reward": z(T * E, torch.float64),
+                        "action": z(T * E, torch.int64) if action_dim is None else
+                        z((T * E, int(action_dim)), torch.float32), "reward": z(T * E, torch.float64),
                         "game_over": z(T * E, torch.uint8)}
         self._stage_dev = {k: torch.zeros((E,) + tuple(v.shape[1:]), dtype=v.dtype, device=dev)
                            for k, v in self.rollout.items()}
@@ -105,10 +107,15 @@ class LockstepSegments(object):
         keep = rows > 0
         return streams[keep], rows[keep]
 
-    def tables(self, streams, rows):
-        """the row-index and segment tables of the segments ``close`` returned; returns the bucket's rows"""
+    def tables(self, streams, rows, B=None):
+        """the row-index and segment tables of the segments ``close`` returned, for a bucket of B rows (default: n
+        rounded up to 32); returns B.  Only the slots a step of B rows reads are written and copied: the B row slots
+        (padding rows read slot 0) and the bootstrap slots."""
         E, T, t_last = self.num_envs, self.t_max, self.t - 1
         n = int(rows.sum())
+        B = round32(n) if B is None else int(B)
+        if B < n or B > self.max_rows:
+            raise ValueError("a bucket of %d rows for %d rows (at most %d)" % (B, n, self.max_rows))
         offsets = np.concatenate([[0], np.cumsum(rows)[:-1]]).astype(np.int64)
         # row j of segment s is the lock-step t_last - rows[s] + 1 + j of its stream
         seg_of_row = np.repeat(np.arange(len(streams)), rows)
@@ -117,23 +124,26 @@ class LockstepSegments(object):
         if self._tab_ev is not None:
             self._tab_ev.synchronize()
         idx, seg = self._idx_host.numpy(), self._seg_host.numpy()
-        idx[:] = 0
+        R = self.max_rows
         idx[:n] = (steps % T) * E + streams[seg_of_row]
-        idx[self.max_rows:self.max_rows + len(streams)] = (t_last % T) * E + streams
+        idx[n:B] = 0
+        idx[R:R + E] = 0
+        idx[R:R + len(streams)] = (t_last % T) * E + streams
         seg[:] = 0
         seg[:len(streams)] = offsets
         seg[E:E + len(streams)] = rows
-        self.idx_dev.copy_(self._idx_host, non_blocking=True)
+        self.idx_dev[:B].copy_(self._idx_host[:B], non_blocking=True)
+        self.idx_dev[R:].copy_(self._idx_host[R:], non_blocking=True)
         self.seg_dev.copy_(self._seg_host, non_blocking=True)
         self._tab_ev = torch.cuda.Event()
         self._tab_ev.record()
-        return round32(n)
+        return B
 
-    def load(self, batch, boot=True):
+    def load(self, batch, boot=True, B=None):
         """given segments, bypassing the rollout buffer: batch is a dict of host arrays states / next_states / actions
         / rewards / game_overs over the rows, and "lengths": the segments' lengths in row order (at most num_envs of
         them).  Fills the learn buffers, the bootstrap states (``boot``) and the segment table; returns the bucket's
-        rows."""
+        rows (B, default n rounded up to 32)."""
         lengths = np.asarray(batch["lengths"], dtype=np.int64)
         n, S = int(lengths.sum()), len(lengths)
         if S < 1 or S > self.num_envs or n > self.max_rows or (lengths < 1).any():
@@ -151,7 +161,10 @@ class LockstepSegments(object):
         seg[:S] = np.concatenate([[0], np.cumsum(lengths)[:-1]])
         seg[self.num_envs:self.num_envs + S] = lengths
         self.seg_dev.copy_(torch.from_numpy(seg))
-        return round32(n)
+        B = round32(n) if B is None else int(B)
+        if B < n or B > self.max_rows:
+            raise ValueError("a bucket of %d rows for %d rows (at most %d)" % (B, n, self.max_rows))
+        return B
 
     def gather(self, B, keys, boot, stream):
         """rows of the closed segments (columns ``keys``) into the learn buffers, and with ``boot`` each segment's last

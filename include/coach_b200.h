@@ -600,6 +600,85 @@ int cb200_actor_critic_head(const cb200_actor_critic_head_desc* ac_desc, void* s
 int cb200_categorical_act(const float* z, int64_t envs, int32_t n_actions, const double* uniforms, int64_t* actions,
                           float* probs, void* stream);
 
+/* Policy gradient targets (agents/policy_gradients_agent.py:47-67, policy_optimization_agent.py:58-71) over a segment
+ * table of whole episodes (the table of cb200_nstep_q_head: slot s covers rows [seg_offsets[s], + seg_lengths[s]),
+ * length 0 = unused), given each row's fp64 return R (cb200_nstep_returns with n_step -1).  Per row, in fp64 with every
+ * operation rounded on its own, then rounded to fp32 into targets:
+ *   TOTAL_RETURN            R_0 of the row's episode
+ *   FUTURE_RETURN           R_i
+ *   NORMALIZED_BY_EPISODE   (R_i - mean) / std, mean and std = np.mean / np.std (population) of the episode's returns
+ *                           with numpy's pairwise summation, bit-identical; 0 when std == 0.  episode_stats (optional,
+ *                           [segments, 2]) receives (mean, std) per slot.
+ *   NORMALIZED_BY_TIMESTEP  R_i - m_i: the episodes are folded in slot order into the running-mean table (table_mean,
+ *                           table_count [table_len], fp64, updated in place): n_i += 1; m_i -= m_i / n_i;
+ *                           m_i += R_i / n_i, and m_i is the table right after the row's own episode was folded.
+ *                           baselines (optional, [rows]) receives that m_i.  A row at a timestep >= table_len gets NaN
+ *                           and leaves the table alone.
+ * Rows covered by no segment are not written. */
+#define CB200_PG_TOTAL_RETURN 0
+#define CB200_PG_FUTURE_RETURN 1
+#define CB200_PG_NORMALIZED_BY_EPISODE 2
+#define CB200_PG_NORMALIZED_BY_TIMESTEP 3
+int cb200_pg_targets(const double* returns, const int32_t* seg_offsets, const int32_t* seg_lengths, int32_t segments,
+                     int64_t rows, int32_t rescaler, double* table_mean, double* table_count, int32_t table_len,
+                     float* targets, double* baselines, double* episode_stats, void* stream);
+
+/* Fused policy gradient head (heads/policy_head.py:54-150, policy_gradients_agent.py:69-86): ONE Dense(n_outputs) on
+ * one feature layer, over the segment table above (segments must not overlap; rows covered by no segment get zero
+ * outputs and dh).  With t_i the row's target and c = 1 / L for an episode of L rows:
+ *   discrete    p = softmax(z) with cb200_actor_critic_head's code, Categorical(probs = p + eps) semantics:
+ *               l_i = c (-log pi(a_i) t_i - beta_entropy H_i); an action outside [0, n_outputs) has no policy term.
+ *   continuous  mean = tanh(z) * max_abs_range (fp32), MultivariateNormalDiag(mean, 1) (the std is the all-ones
+ *               policy_stdev variable): log pi(x) = -|x - mean|^2 / 2 - D log(2 pi) / 2, H = D (1 + log(2 pi)) / 2
+ *               (no gradient); l_i = c (-log pi(x_i) t_i - beta_entropy H).
+ *   loss = sum_i l_i: the sum over the table's episodes of each episode's mean loss, and dz = dL/dZ, so the gradient
+ *   is the sum of the episodes' gradients (what accumulate_gradients adds up).  dW = h^T dz, db = sum_i dz_i,
+ *   dh = (dz W^T) relu'(h).
+ * Parallel over rows; dW, db and the loss are summed per 64-row chunk, then over the chunks in a fixed order: no
+ * atomics, repeat calls and graph replays give the same bits.  features 256 or 512; n_outputs <= 18 (discrete) or
+ * <= 32 (continuous). */
+typedef struct cb200_policy_gradient_head_desc {
+    const float* h;             /* [rows, features] post-ReLU features                                                   */
+    const float* w;             /* head kernel [features, n_outputs] and bias [n_outputs]                                */
+    const float* b;
+    const float* targets;       /* [rows] (cb200_pg_targets)                                                             */
+    const int64_t* actions;     /* [rows], discrete                                                                      */
+    const float* cont_actions;  /* [rows, n_outputs], continuous                                                         */
+    const float* max_abs_range; /* [n_outputs], continuous                                                               */
+    const int32_t* seg_offsets; /* [segments]                                                                            */
+    const int32_t* seg_lengths; /* [segments], 0 = unused slot                                                           */
+    int32_t segments;           /* 1 .. 2^20                                                                              */
+    int64_t rows;               /* rows of the feature / output buffers, 1 .. 2^24                                       */
+    int32_t continuous;         /* 0 discrete (Categorical), 1 bounded Gaussian                                          */
+    int32_t features;           /* 256 or 512                                                                             */
+    int32_t n_outputs;          /* actions (discrete) or action dimensions (continuous)                                  */
+    float beta_entropy;
+    float* z;                   /* out [rows, n_outputs]: the Dense outputs (logits / pre-tanh means)                    */
+    float* policy;              /* out, optional [rows, n_outputs]: p (discrete) or the mean (continuous)                */
+    float* dz;                  /* out, optional [rows, n_outputs]: dL/dZ                                                */
+    float* loss;                /* out scalar, optional                                                                   */
+    float* dh;                  /* out, optional: [rows, features] dL/d(pre-activation of the feature layer)             */
+    void* dh_planes;            /* out, optional: the same as tiled bf16 hi / mid / lo planes                             */
+    int64_t dh_plane_stride;
+    float* dw;                  /* out [features, n_outputs]                                                             */
+    float* db;                  /* out [n_outputs]                                                                        */
+    float* workspace;           /* rows * (n_outputs + 1) + ceil(rows / 64) * (features * n_outputs + n_outputs + 1)    */
+} cb200_policy_gradient_head_desc;
+
+int cb200_policy_gradient_head(const cb200_policy_gradient_head_desc* pg_desc, void* stream);
+
+/* Acting from a policy gradient head's outputs z [envs, n_outputs]:
+ *   discrete    cb200_categorical_act's softmax and draw (uniforms in `draws` [envs], NULL: the first argmax) into
+ *               actions [envs], probs [envs, n_outputs] optional.
+ *   continuous  AdditiveNoise (exploration_policies/additive_noise.py:74-103): mean = tanh(z) * max_abs_range (fp32, the
+ *               head's code); with draws [envs, n_outputs] (np.random.standard_normal) the action is numpy's
+ *               normal(mean, scale) = (double) mean + scale[e, d] * draw in fp64 (scale [envs, n_outputs] fp64: each
+ *               environment's noise times high - low); draws NULL (evaluation): the mean.  cont_actions [envs, n_outputs] fp64 out, means
+ *               [envs, n_outputs] fp32 optional. */
+int cb200_policy_act(const float* z, int64_t envs, int32_t n_outputs, int32_t continuous, const float* max_abs_range,
+                     const double* draws, const double* scale, int64_t* actions, float* probs, double* cont_actions,
+                     float* means, void* stream);
+
 /* Acting values of an ensemble, q [envs, heads * n_actions] -> out [envs, n_actions], in the exploration policies' fp32
  * numpy arithmetic (exploration_policies/bootstrapped.py:70-84, ucb.py:70-83):
  *   SELECT  the row of head[e] (Bootstrapped, training)
