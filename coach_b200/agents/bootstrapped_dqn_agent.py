@@ -123,12 +123,7 @@ class BootstrappedDQNAgent(DQNAgent):
         d.grad_rescale = self.grad_rescale
         d.q_online, d.dq = on.q.data_ptr(), on.dq.data_ptr()
         d.q_next, d.q_select = net.target_s2.q.data_ptr(), self.q_select.data_ptr()
-        dz = on.trunk.dzs[-2]
-        d.dh = dz.data_ptr() if dz is not None else None
-        pl = on.trunk.dz_planes[-2]
-        if pl is not None:
-            d.dh_planes, d.dh_plane_stride = pl.ptr, pl.stride
-        d.dw, d.db = store.view(store.grad, wname).data_ptr(), store.view(store.grad, bname).data_ptr()
+        on.bind_head_grads(d)
         d.workspace = self._head_keep[0].data_ptr()
         self.head_desc = d
 

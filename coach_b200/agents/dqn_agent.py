@@ -133,12 +133,12 @@ class QNetworkWrapper(object):
         if self.theta_target is not None:
             self._refresh(self.theta_target)
 
-    def apply_gradients(self, scaler=1.0):
+    def apply_gradients(self, scaler=1.0, grad=None):
         """clip is applied by the caller (accumulate_gradients side in the reference); here: optional rescale,
-        then the optimizer (architecture.py:469-521)."""
+        then the optimizer (architecture.py:469-521).  grad: the gradient buffer to apply, default ``store.grad``."""
         st = _lib.current_stream()
         n = self.store.size
-        grad = self.store.grad
+        grad = self.store.grad if grad is None else grad
         if scaler != 1.0:
             _lib.check(self.lib.cb200_scale(grad.data_ptr(), n, float(scaler), st))
         p = self.params
@@ -340,12 +340,7 @@ class DQNAgent(object):
         d.batch, d.features, d.n_actions = B, K, A
         d.q_online, d.dq = on.q.data_ptr(), on.dq.data_ptr()
         d.q_next = net.target_s2.q.data_ptr()
-        dz = on.trunk.dzs[-2]
-        d.dh = dz.data_ptr() if dz is not None else None
-        pl = on.trunk.dz_planes[-2]
-        if pl is not None:
-            d.dh_planes, d.dh_plane_stride = pl.ptr, pl.stride
-        d.dw, d.db = store.view(store.grad, wname).data_ptr(), store.view(store.grad, bname).data_ptr()
+        on.bind_head_grads(d)
         d.workspace = self._head_keep[0].data_ptr()
         # descriptor field -> batch column, pointed at the step's batch before every head launch
         self._head_columns = {"actions": "action", "rewards": "reward", "game_overs": "game_over"}

@@ -11,12 +11,10 @@ segments of each segment's own gradient (the synchronous-training rule of
 lock-step steps (each stream's own steps); ``training_iteration`` counts learn steps.  With E = 1 this is the
 reference schedule.
 
-The rollout buffer, the cuts, the gather and the 32-row buckets with their CUDA graphs are
-``coach_b200.memories.lockstep_segments``.
-
-One learn step = gather -> target features of the bootstrap states (N-Step) or of every s' (1-Step) -> online features
--> ``cb200_nstep_q_head`` (Q, bootstrap max, the fp64 return recurrence, targets, loss, dL/dQ, the head's gradients and
-dL/dh) -> backward -> TF-Adam.  Every 32-row bucket has its own forward / backward instance on the shared parameters.
+The rollout buffer, the cuts and the gather are ``coach_b200.memories.lockstep_segments``, the row buckets and the
+learn step's skeleton ``coach_b200.agents.lockstep_agent``.  One learn step = gather -> target features of the bootstrap
+states (N-Step) or of every s' (1-Step) -> online features -> ``cb200_nstep_q_head`` (Q, bootstrap max, the fp64
+return recurrence, targets, loss, dL/dQ, the head's gradients and dL/dh) -> backward -> TF-Adam.
 
 Refused (ValueError): ``apply_gradients_every_x_episodes != 1`` (gradients are applied after every segment), a
 ``targets_horizon`` other than 'N-Step' / '1-Step' (the reference silently trains on zero loss then), a dueling head, and
@@ -26,17 +24,13 @@ from the rows observed since.
 """
 import ctypes
 
-import numpy as np
-import torch
-
 from coach_b200 import _lib, parallel
-from coach_b200.agents.dqn_agent import DQNAgent, QNetworkWrapper
+from coach_b200.agents.dqn_agent import DQNAgent
+from coach_b200.agents.lockstep_agent import LockstepAgent
 from coach_b200.architectures.layers import Workspace
-from coach_b200.architectures.q_network import QNetworkDef
 from coach_b200.base_parameters import (AgentParameters, AlgorithmParameters, EnvironmentSteps,
-                                        InputEmbedderParameters, NetworkParameters, middleware_units, scheme_layers)
+                                        InputEmbedderParameters, NetworkParameters)
 from coach_b200.exploration_policies.e_greedy import EGreedyParameters
-from coach_b200.memories.lockstep_segments import LockstepSegments
 
 HORIZONS = {"N-Step": _lib.NSTEP_NSTEP, "1-Step": _lib.NSTEP_ONESTEP}
 
@@ -78,10 +72,15 @@ class NStepQAgentParameters(AgentParameters):
         return 'coach_b200.agents.n_step_q_agent:NStepQAgent'
 
 
-class NStepQAgent(object):
+class NStepQAgent(LockstepAgent):
+    head_desc_type = _lib.NstepQHeadDesc
+    head_error = "cb200_nstep_q_head needs a QHead of <= 18 actions on a 256- or 512-wide ReLU layer"
+    graph_tuning = "nstep_graph"
+    is_on_policy = False
+
     def __init__(self, agent_parameters, parent=None, observation_shape=None, num_actions=None, num_envs=1,
                  device=None, seed=None):
-        self.ap = ap = agent_parameters
+        ap = agent_parameters
         alg, net_params = ap.algorithm, ap.network_wrappers["main"]
         if alg.apply_gradients_every_x_episodes != 1:
             raise ValueError("apply_gradients_every_x_episodes must be 1: gradients are applied after every segment")
@@ -92,72 +91,25 @@ class NStepQAgent(object):
             raise ValueError("NStepQAgent takes a plain QHead, not a dueling head")
         if parallel.is_distributed():
             raise ValueError("NStepQAgent runs on one rank")
-        self.parent = parent
-        self.lib = _lib.load()
-        self.device = dev = torch.device(device if device is not None else "cuda")
-        self.observation_shape = obs = tuple(observation_shape if observation_shape is not None
-                                             else ap.observation_shape)
-        self.num_actions = A = int(num_actions if num_actions is not None else ap.num_actions)
-        self.num_envs = E = int(num_envs)
-        self.t_max = int(alg.num_steps_between_gradient_updates)
+        self.num_actions = int(num_actions if num_actions is not None else ap.num_actions)
         self.horizon = HORIZONS[alg.targets_horizon]
-        emb = getattr(net_params, "input_embedders_parameters", {}).get("observation")
-        scheme = getattr(getattr(net_params, "middleware_parameters", None), "scheme", "Medium")
-        self.net_def = QNetworkDef(dev, obs, A, middleware_units=middleware_units(scheme),
-                                   embedder_scheme=scheme_layers(getattr(emb, "scheme", "Medium")))
-        gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
-        self.net_def.store.init_glorot(gen)
-        self.segments = sg = LockstepSegments(self.lib, dev, obs, E, self.t_max)
-        self.learn, self.boot_states, self.max_rows = sg.learn, sg.boot_states, sg.max_rows
-        # the shared parameters (online, target, Adam) and the acting path of the DQN agent.  The wrapper's own
-        # bindings are the 32-row bucket.
-        self.batch_buffers = {"state:observation": self.learn["state"][:32],
-                              "next_state:observation": self.learn["next_state"][:32]}
-        self.networks = {"main": QNetworkWrapper(self.lib, self.net_def, net_params, 32, self.batch_buffers, False,
-                                                 dev)}
+        self.gather_keys = ("state", "action", "reward", "game_over") + \
+            (("next_state",) if self.horizon == _lib.NSTEP_ONESTEP else ())
+        self.gather_boot = self.horizon == _lib.NSTEP_NSTEP
+        super().__init__(ap, parent, observation_shape, num_envs, device, seed, self.num_actions)
         net = self.networks["main"]
         net.sync()
         self.target_boot = None
         if self.horizon == _lib.NSTEP_NSTEP:
-            self.target_boot = self.net_def.instantiate(self.lib, Workspace(dev), E, self.boot_states,
-                                                        net.theta_target)
+            self.target_boot = self.net_def.instantiate(self.lib, Workspace(self.device), self.num_envs,
+                                                        self.segments.boot_states, net.theta_target)
             net.add_planes(self.target_boot)
-        self._buckets = {}
-        self.loss_dev = torch.zeros(1, dtype=torch.float32, device=dev)
-        self._fetch_host = torch.zeros(2, dtype=torch.float32, pin_memory=dev.type == "cuda")
-        self._acting = {}
-        # counters of agents/agent.py:112-135
-        self.training_iteration = 0
-        self.total_steps_counter = 0
         self.last_target_network_update_step = 0
 
-    # ---- reference plumbing and the DQN agent's acting path -------------------------------------------------------------
-    @property
-    def is_on_policy(self) -> bool:
-        return False
-
+    # ---- the DQN agent's acting path ----------------------------------------------------------------------------------------
     _should_update_online_weights_to_target = DQNAgent._should_update_online_weights_to_target
     get_all_q_values_for_states = DQNAgent.get_all_q_values_for_states
     choose_actions = DQNAgent.choose_actions
-
-    def _join_optimizer(self):
-        pass                                                   # the optimizer runs on the caller's stream
-
-    @property
-    def learned_segments(self):
-        """(stream, start, end) of the segments the last train() step learned"""
-        return self.segments.learned_segments
-
-    @property
-    def graph_kernel_launches(self):
-        return self.segments.graph_kernel_launches
-
-    # ---- rollout ----------------------------------------------------------------------------------------------------------
-    def observe_batch(self, states, actions, rewards, next_states, game_overs):
-        """one lock-step of the E streams (agent.py:820-834 act's step count, :905-975 observe, core_types.py:716-725
-        Episode.insert): host arrays [E, ...]"""
-        self.segments.observe(states, actions, rewards, next_states, game_overs)
-        self.total_steps_counter += 1
 
     def train(self, fetch=True):
         """n_step_q_agent.py:142-153 + policy_optimization_agent.py:85-135: target copy check first, then one learn step
@@ -172,102 +124,34 @@ class NStepQAgent(object):
         return self._learn(self.segments.tables(streams, rows), True, fetch)
 
     # ---- the learn step ---------------------------------------------------------------------------------------------------
-    def learn_from_batch(self, batch, fetch=True):
-        """one learn step on given segments, bypassing the rollout buffer.  batch: dict of host arrays
-        states / next_states / actions / rewards / game_overs over the rows, and "lengths": the segments' lengths in row
-        order (at most num_envs of them).  Returns (loss, [loss], unclipped gradient norm) with fetch, else device
-        scalars."""
-        B = self.segments.load(batch, boot=self.horizon == _lib.NSTEP_NSTEP)
-        return self._learn(B, False, fetch)
-
-    def _bucket(self, B):
-        bk = self._buckets.get(B)
-        if bk is not None:
-            return bk
-        lib, dev, net, nd = self.lib, self.device, self.networks["main"], self.net_def
-        if B == 32:
-            on = net.online_s
-            tn = net.target_s2
-        else:
-            on = nd.instantiate(lib, Workspace(dev), B, self.learn["state"][:B], net.theta, net.store.grad, train=True)
-            tn = None
-            if self.horizon == _lib.NSTEP_ONESTEP:
-                tn = nd.instantiate(lib, Workspace(dev), B, self.learn["next_state"][:B], net.theta_target)
-                net.add_planes(tn)
+    def _boot_instance(self, B):
+        """the target network on the bootstrap states (N-Step) or on every row's s' (1-Step)"""
+        net = self.networks["main"]
         if self.horizon == _lib.NSTEP_NSTEP:
-            tn = self.target_boot
-        head = on.trunk.layers[-1]
-        if not (not nd.dueling and len(on.trunk.layers) >= 2 and type(head).__name__ == "Dense" and
-                head.K in (256, 512) and head.N == self.num_actions <= 18 and on.trunk.acts[-2] is not None and
-                on.trunk.layers[-2].act == 1 and tn.trunk.acts[-2] is not None):
-            raise ValueError("cb200_nstep_q_head needs a QHead of <= 18 actions on a 256- or 512-wide ReLU layer")
-        store = net.store
-        wname, bname = nd.trunk.names[-1]
-        K, A, E = head.K, self.num_actions, self.num_envs
-        d = _lib.NstepQHeadDesc()
-        keep = torch.zeros(((E + 3) // 4) * 4 * (K * A + A + 1), dtype=torch.float32, device=dev)
+            return self.target_boot
+        if B == 32:
+            return net.target_s2
+        tn = self.net_def.instantiate(self.lib, Workspace(self.device), B, self.learn["next_state"][:B],
+                                      net.theta_target)
+        net.add_planes(tn)
+        return tn
+
+    def _fill_desc(self, d, on, tn, B):
+        net, store, alg = self.networks["main"], self.net_def.store, self.ap.algorithm
+        wname, bname = self.net_def.trunk.names[-1]
         d.h_online, d.h_boot = on.trunk.acts[-2].data_ptr(), tn.trunk.acts[-2].data_ptr()
         d.w_target, d.b_target = store.view(net.theta_target, wname).data_ptr(), \
             store.view(net.theta_target, bname).data_ptr()
         d.w_online, d.b_online = store.view(net.theta, wname).data_ptr(), store.view(net.theta, bname).data_ptr()
         d.actions, d.rewards = self.learn["action"].data_ptr(), self.learn["reward"].data_ptr()
         d.game_overs = self.learn["game_over"].data_ptr()
-        d.seg_offsets, d.seg_lengths = self.segments.seg_table()
-        d.segments, d.rows = E, B
-        d.discount = float(self.ap.algorithm.discount)
+        d.discount = float(alg.discount)
         d.horizon = self.horizon
         d.huber = 1 if net.params.replace_mse_with_huber_loss else 0
-        d.features, d.n_actions = K, A
-        d.q_online, d.dq, d.loss = on.q.data_ptr(), on.dq.data_ptr(), self.loss_dev.data_ptr()
-        dz = on.trunk.dzs[-2]
-        d.dh = dz.data_ptr() if dz is not None else None
-        pl = on.trunk.dz_planes[-2]
-        if pl is not None:
-            d.dh_planes, d.dh_plane_stride = pl.ptr, pl.stride
-        d.dw, d.db = store.view(store.grad, wname).data_ptr(), store.view(store.grad, bname).data_ptr()
-        d.workspace = keep.data_ptr()
-        bk = self._buckets[B] = (on, tn, d, keep)
-        return bk
+        d.n_actions = self.num_actions
+        d.q_online, d.dq = on.q.data_ptr(), on.dq.data_ptr()
+        K, A, E = d.features, self.num_actions, self.num_envs
+        return ((E + 3) // 4) * 4 * (K * A + A + 1)
 
-    def _device_step(self, B, gather):
-        lib, st = self.lib, _lib.current_stream()
-        net = self.networks["main"]
-        on, tn, d, _ = self._bucket(B)
-        if gather:
-            keys = ("state", "action", "reward", "game_over") + \
-                (("next_state",) if self.horizon == _lib.NSTEP_ONESTEP else ())
-            self.segments.gather(B, keys, self.horizon == _lib.NSTEP_NSTEP, st)
-        if on.theta_planes is not None and on is not net.online_s:
-            on.theta_planes.refresh()                          # this bucket's operand planes of the current theta
-        tn.forward_features()
-        on.forward_features()
-        _lib.check(lib.cb200_nstep_q_head(ctypes.byref(d), st))
-        on.backward_features()
-        _lib.check(lib.cb200_sumsq(net.store.grad.data_ptr(), net.store.size, net.sumsq.data_ptr(), net.ws.ptr(), st))
-        clip = net.params.clip_gradients
-        if clip is not None and clip != 0:
-            if net.params.gradients_clipping_method != "ClipByGlobalNorm":
-                raise NotImplementedError("only ClipByGlobalNorm is implemented on device")
-            _lib.check(lib.cb200_clip_by_global_norm(net.store.grad.data_ptr(), net.store.size, net.sumsq.data_ptr(),
-                                                     float(clip), st))
-        net.apply_gradients(1.0)
-
-    def _learn(self, B, gather, fetch):
-        self.segments.run(B, gather, self._device_step, _lib.tune_default("nstep_graph", 1))
-        if not fetch:
-            return self.loss_dev if gather else (self.loss_dev, [self.loss_dev], self.networks["main"].sumsq)
-        self._fetch_host[0:1].copy_(self.loss_dev, non_blocking=True)
-        self._fetch_host[1:2].copy_(self.networks["main"].sumsq, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        loss = float(self._fetch_host[0])
-        if gather:
-            return loss
-        return loss, [loss], float(np.sqrt(np.float32(self._fetch_host[1])))
-
-    # ---- checkpoints (coach_b200/checkpoint.py) -------------------------------------------------------------------------
-    def checkpoint_state(self):
-        """every stream's cut position; the rows of open segments are not saved"""
-        return self.segments.state()
-
-    def restore_checkpoint_state(self, state):
-        self.segments.restore(state)
+    def _launch_head(self, d, st):
+        _lib.check(self.lib.cb200_nstep_q_head(ctypes.byref(d), st))

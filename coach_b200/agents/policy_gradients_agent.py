@@ -29,10 +29,9 @@ reference loses its open episode the same way (a restored worker starts a new on
 Learn steps run on row buckets: 32-row steps up to 256 rows, then four sizes per doubling (at most 25 % padding), which
 bounds the number of per-bucket network instances and CUDA graphs to about 4 log2(rows / 256) + 8.
 
-One learn step = gather -> ``cb200_nstep_returns`` (n_step -1) -> ``cb200_pg_targets`` (the rescaler, the device table
-of the timestep rescaler) -> online features of the rows -> ``cb200_policy_gradient_head`` -> backward ->
-``cb200_axpby_2d`` into the accumulator.  Every 32-row bucket has its own forward / backward instance; from 128 rows on a
-bucket's step is replayed as one CUDA graph.  The apply decision stays on the host.
+One learn step = gather -> online features of the rows -> ``cb200_nstep_returns`` (n_step -1) -> ``cb200_pg_targets``
+(the rescaler, the device table of the timestep rescaler) -> ``cb200_policy_gradient_head`` -> backward ->
+``cb200_axpby_2d`` into the accumulator (coach_b200.agents.lockstep_agent).  The apply decision stays on the host.
 
 Refused (ValueError): a rescaler other than the four return-based ones, ``n_step != -1``, ``clip_gradients`` (the
 reference clips each episode's gradient before accumulating it, which one backward pass over several episodes cannot
@@ -47,12 +46,9 @@ import torch
 
 from coach_b200 import _lib, parallel
 from coach_b200.agents.actor_critic_agent import CategoricalParameters, PolicyGradientRescaler
-from coach_b200.agents.dqn_agent import DQNAgent, QNetworkWrapper
-from coach_b200.architectures.layers import Workspace
-from coach_b200.architectures.q_network import QNetworkDef
-from coach_b200.base_parameters import (AgentParameters, AlgorithmParameters, InputEmbedderParameters,
-                                        NetworkParameters, middleware_units, scheme_layers)
-from coach_b200.memories.lockstep_segments import LockstepSegments, round32
+from coach_b200.agents.lockstep_agent import LockstepAgent
+from coach_b200.base_parameters import AgentParameters, AlgorithmParameters, InputEmbedderParameters, NetworkParameters
+from coach_b200.memories.lockstep_segments import round32
 from coach_b200.schedules import LinearSchedule
 
 __all__ = ["PolicyGradientRescaler", "PolicyGradientAlgorithmParameters", "PolicyGradientNetworkParameters",
@@ -132,12 +128,18 @@ def _unpack(s, t):
     t.copy_(torch.from_numpy(np.frombuffer(base64.b64decode(s), dtype=t.cpu().numpy().dtype).copy()))
 
 
-class PolicyGradientsAgent(object):
+class PolicyGradientsAgent(LockstepAgent):
+    head_desc_type = _lib.PolicyGradientHeadDesc
+    head_error = ("cb200_policy_gradient_head needs <= 18 actions (<= 32 action dimensions) on a 256- or 512-wide ReLU "
+                  "layer")
+    graph_tuning = "pg_graph"
+    gather_keys, gather_boot = ("state", "action", "reward"), False
+
     def __init__(self, agent_parameters, parent=None, observation_shape=None, num_actions=None, num_envs=1,
                  device=None, seed=None, action_dim=None, action_low=None, action_high=None):
         """num_actions: a discrete action space; or action_dim with the bounds action_low / action_high [action_dim]
         (a BoxActionSpace: gym's float32 arrays)"""
-        self.ap = ap = agent_parameters
+        ap = agent_parameters
         alg, net_params = ap.algorithm, ap.network_wrappers["main"]
         if alg.policy_gradient_rescaler not in RESCALERS:
             raise ValueError("policy_gradient_rescaler must be TOTAL_RETURN, FUTURE_RETURN or one of the two "
@@ -150,6 +152,7 @@ class PolicyGradientsAgent(object):
         if parallel.is_distributed():
             raise ValueError("PolicyGradientsAgent runs on one rank")
         self.continuous = action_dim is not None
+        self.max_outputs = 32 if self.continuous else 18
         if self.continuous:
             if action_low is None or action_high is None:
                 raise ValueError("continuous actions need the bounds action_low / action_high")
@@ -158,34 +161,17 @@ class PolicyGradientsAgent(object):
                 raise ValueError("Additive noise exploration requires bounded actions")
         elif num_actions is None and getattr(ap, "num_actions", None) is None:
             raise ValueError("give num_actions (discrete) or action_dim with its bounds (continuous)")
-        self.parent = parent
-        self.lib = _lib.load()
-        self.device = dev = torch.device(device if device is not None else "cuda")
-        self.observation_shape = obs = tuple(observation_shape if observation_shape is not None
-                                             else ap.observation_shape)
         self.num_outputs = N = int(action_dim) if self.continuous else \
             int(num_actions if num_actions is not None else ap.num_actions)
         self.num_actions = None if self.continuous else N
-        self.num_envs = E = int(num_envs)
-        self.t_max = int(alg.num_steps_between_gradient_updates)
         self.every = int(alg.apply_gradients_every_x_episodes)
         if self.every < 1:
             raise ValueError("apply_gradients_every_x_episodes must be >= 1")
         self.rescaler = RESCALERS[alg.policy_gradient_rescaler]
-        emb = getattr(net_params, "input_embedders_parameters", {}).get("observation")
-        scheme = getattr(getattr(net_params, "middleware_parameters", None), "scheme", "Medium")
-        self.net_def = QNetworkDef(dev, obs, N, middleware_units=middleware_units(scheme),
-                                   embedder_scheme=scheme_layers(getattr(emb, "scheme", "Medium")))
-        gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
-        self.net_def.store.init_glorot(gen)
-        self.segments = sg = LockstepSegments(self.lib, dev, obs, E, self.t_max, N if self.continuous else None)
-        self.learn = sg.learn
-        self.batch_buffers = {"state:observation": self.learn["state"][:32],
-                              "next_state:observation": self.learn["next_state"][:32]}
-        self.networks = {"main": QNetworkWrapper(self.lib, self.net_def, net_params, 32, self.batch_buffers, False,
-                                                 dev)}
-        store = self.net_def.store
-        self.accumulator = torch.zeros(store.size, dtype=torch.float32, device=dev)
+        super().__init__(ap, parent, observation_shape, num_envs, device, seed, N,
+                         action_dim=N if self.continuous else None)
+        dev, E, sg = self.device, self.num_envs, self.segments
+        self.accumulator = torch.zeros(self.net_def.store.size, dtype=torch.float32, device=dev)
         # the per-timestep running mean of update_episode_statistics (mean, count), over t_max timesteps
         self.table = torch.zeros((2, self.t_max), dtype=torch.float64, device=dev)
         # a part holds at most x whole episodes
@@ -201,45 +187,19 @@ class PolicyGradientsAgent(object):
             self.max_abs_range = torch.from_numpy(rng).to(dev)
             ex = ap.exploration["BoxActionSpace"] if isinstance(ap.exploration, dict) else ap.exploration
             self.noise_schedule = ex.noise_schedule
-        self._buckets = {}
-        self.loss_dev = torch.zeros(1, dtype=torch.float32, device=dev)
-        self._fetch_host = torch.zeros(1, dtype=torch.float32, pin_memory=pin)
-        self._acting = {}
         self._act_out = {}
-        # counters of agents/agent.py:112-135
         self.current_episode = 0
-        self.training_iteration = 0
-        self.total_steps_counter = 0
         self.last_parts = []                                   # [(episodes, applied)] of the last train()
         self._learned = []
         # streams whose open episode was cut by a checkpoint restore: discarded until their next game_over
         self.discard = np.zeros(E, dtype=bool)
-
-    # ---- reference plumbing -------------------------------------------------------------------------------------------------
-    @property
-    def is_on_policy(self) -> bool:
-        return True
-
-    def _join_optimizer(self):
-        pass                                                   # the optimizer runs on the caller's stream
 
     @property
     def learned_segments(self):
         """(stream, start, end) of the episodes the last train() step learned"""
         return self._learned
 
-    @property
-    def graph_kernel_launches(self):
-        return self.segments.graph_kernel_launches
-
-    # ---- acting -------------------------------------------------------------------------------------------------------------
-    _forward_acting = DQNAgent.get_all_q_values_for_states
-
-    def get_prediction(self, states):
-        """the head's Dense outputs [E, N] for E states (logits, or the pre-tanh means) as a CUDA tensor (persistent
-        buffer, valid until the next call)"""
-        return self._forward_acting(states)
-
+    # ---- acting (get_prediction: [E, N] outputs, the logits or the pre-tanh means) ----------------------------------------
     def choose_actions(self, states, evaluation=False, draws=None):
         """policy_optimization_agent.py:143-160 for E environments.
         Discrete: Categorical.get_action per environment: np.random.choice(A, p=softmax) on ``draws`` [E] (default
@@ -275,10 +235,7 @@ class PolicyGradientsAgent(object):
                 out["scale"].copy_(torch.from_numpy(scale))
             else:
                 d = np.random.random_sample(E) if draws is None else np.asarray(draws, dtype=np.float64)
-            torch.cuda.current_stream().synchronize()          # the previous call's copy has left the staging
-            out["d_host"].numpy()[...] = d.reshape(out["d_host"].shape)
-            out["d_dev"].copy_(out["d_host"], non_blocking=True)
-            d_ptr = out["d_dev"].data_ptr()
+            d_ptr = self._stage(out["d_host"], out["d_dev"], d)
         rng = self.max_abs_range.data_ptr() if self.continuous else None
         _lib.check(self.lib.cb200_policy_act(z.data_ptr(), E, N, int(self.continuous), rng, d_ptr,
                                              out["scale"].data_ptr(), out["actions"].data_ptr(),
@@ -288,13 +245,6 @@ class PolicyGradientsAgent(object):
             return out["actions"].cpu().numpy(), out["probs"].cpu().numpy()
         means = out["probs"].cpu().numpy()
         return (means.copy() if evaluation else out["cont"].cpu().numpy()), means
-
-    # ---- rollout ------------------------------------------------------------------------------------------------------------
-    def observe_batch(self, states, actions, rewards, next_states, game_overs):
-        """one lock-step of the E streams (agent.py:905-975 observe, core_types.py:716-725 Episode.insert): host
-        arrays [E, ...]"""
-        self.segments.observe(states, actions, rewards, next_states, game_overs)
-        self.total_steps_counter += 1
 
     def train(self, fetch=True):
         """policy_optimization_agent.py:85-135 over the episodes that closed at this lock-step, cut into parts at the
@@ -367,25 +317,9 @@ class PolicyGradientsAgent(object):
             raise ValueError("a learn step of %d rows exceeds the %d-row buffers" % (n, R))
         return min(bucket_rows(n), R)
 
-    def _bucket(self, B):
-        bk = self._buckets.get(B)
-        if bk is not None:
-            return bk
-        lib, dev, net, nd = self.lib, self.device, self.networks["main"], self.net_def
-        on = net.online_s if B == 32 else \
-            nd.instantiate(lib, Workspace(dev), B, self.learn["state"][:B], net.theta, net.store.grad, train=True)
-        head = on.trunk.layers[-1]
-        N = self.num_outputs
-        if not (len(on.trunk.layers) >= 2 and head.K in (256, 512) and head.N == N and
-                N <= (32 if self.continuous else 18) and on.trunk.acts[-2] is not None and
-                on.trunk.layers[-2].act == 1):
-            raise ValueError("cb200_policy_gradient_head needs <= 18 actions (<= 32 action dimensions) on a 256- or "
-                             "512-wide ReLU layer")
-        store = net.store
-        wname, bname = nd.trunk.names[-1]
-        K = head.K
-        d = _lib.PolicyGradientHeadDesc()
-        keep = torch.zeros(B * (N + 1) + (B + 63) // 64 * (K * N + N + 1), dtype=torch.float32, device=dev)
+    def _fill_desc(self, d, on, boot, B):
+        net, store = self.networks["main"], self.net_def.store
+        wname, bname = self.net_def.trunk.names[-1]
         d.h = on.trunk.acts[-2].data_ptr()
         d.w, d.b = store.view(net.theta, wname).data_ptr(), store.view(net.theta, bname).data_ptr()
         d.targets = self.targets.data_ptr()
@@ -393,63 +327,41 @@ class PolicyGradientsAgent(object):
             d.cont_actions, d.max_abs_range = self.learn["action"].data_ptr(), self.max_abs_range.data_ptr()
         else:
             d.actions = self.learn["action"].data_ptr()
-        d.seg_offsets, d.seg_lengths = self.segments.seg_table()
-        d.segments, d.rows = self.num_envs, B
-        d.continuous, d.features, d.n_outputs = int(self.continuous), K, N
+        N = self.num_outputs
+        d.continuous, d.n_outputs = int(self.continuous), N
         d.beta_entropy = float(self.ap.algorithm.beta_entropy)
-        d.z, d.loss = on.q.data_ptr(), self.loss_dev.data_ptr()
-        dz = on.trunk.dzs[-2]
-        d.dh = dz.data_ptr() if dz is not None else None
-        pl = on.trunk.dz_planes[-2]
-        if pl is not None:
-            d.dh_planes, d.dh_plane_stride = pl.ptr, pl.stride
-        d.dw, d.db = store.view(store.grad, wname).data_ptr(), store.view(store.grad, bname).data_ptr()
-        d.workspace = keep.data_ptr()
-        bk = self._buckets[B] = (on, d, keep)
-        return bk
+        d.z = on.q.data_ptr()
+        return B * (N + 1) + (B + 63) // 64 * (d.features * N + N + 1)
 
-    def _device_step(self, B, gather):
-        lib, st = self.lib, _lib.current_stream()
-        net = self.networks["main"]
-        on, d, _ = self._bucket(B)
-        if gather:
-            self.segments.gather(B, ("state", "action", "reward"), False, st)
-        if on.theta_planes is not None and on is not net.online_s:
-            on.theta_planes.refresh()                          # this bucket's operand planes of the current theta
+    def _launch_head(self, d, st):
+        lib = self.lib
         _lib.check(lib.cb200_nstep_returns(self.learn["reward"].data_ptr(), self.ep_bounds[0].data_ptr(),
-                                           self.ep_bounds[1].data_ptr(), B, float(self.ap.algorithm.discount), -1,
+                                           self.ep_bounds[1].data_ptr(), d.rows, float(self.ap.algorithm.discount), -1,
                                            self.returns.data_ptr(), st))
         off, ln = self.segments.seg_table()
-        _lib.check(lib.cb200_pg_targets(self.returns.data_ptr(), off, ln, self.num_envs, B, self.rescaler,
+        _lib.check(lib.cb200_pg_targets(self.returns.data_ptr(), off, ln, self.num_envs, d.rows, self.rescaler,
                                         self.table[0].data_ptr(), self.table[1].data_ptr(), self.t_max,
                                         self.targets.data_ptr(), None, None, st))
-        on.forward_features()
         _lib.check(lib.cb200_policy_gradient_head(ctypes.byref(d), st))
-        on.backward_features()
-        store = net.store
-        _lib.check(lib.cb200_axpby_2d(store.grad.data_ptr(), store.size, 1, store.size, 1.0, 1.0,
-                                      self.accumulator.data_ptr(), store.size, st))
+
+    def _sink_gradients(self, st):
+        """the step's gradient is added to the accumulator"""
+        store = self.net_def.store
+        _lib.check(self.lib.cb200_axpby_2d(store.grad.data_ptr(), store.size, 1, store.size, 1.0, 1.0,
+                                           self.accumulator.data_ptr(), store.size, st))
 
     def apply_and_reset_gradients(self):
         """architecture.py:469-521 apply_and_reset_gradients: one TF-Adam step on the accumulated sum, then zero it"""
-        net, st = self.networks["main"], _lib.current_stream()
-        p, store = net.params, net.store
-        if p.optimizer_type != 'Adam':
-            raise NotImplementedError("only the Adam optimizer is implemented on device")
-        _lib.check(self.lib.cb200_adam_tf_dev(net.theta.data_ptr(), store.m.data_ptr(), store.v.data_ptr(),
-                                              self.accumulator.data_ptr(), store.size, float(p.learning_rate),
-                                              float(p.adam_optimizer_beta1), float(p.adam_optimizer_beta2),
-                                              float(p.optimizer_epsilon), net.adam_state.data_ptr(), st))
-        net.online_changed()
+        self.networks["main"].apply_gradients(1.0, self.accumulator)
         self.accumulator.zero_()
 
     def _learn(self, B, gather, apply, fetch):
-        self.segments.run(B, gather, self._device_step, _lib.tune_default("pg_graph", 1))
+        self.segments.run(B, gather, self._device_step, _lib.tune_default(self.graph_tuning, 1))
         if apply:
             self.apply_and_reset_gradients()
         if not fetch:
             return self.loss_dev
-        self._fetch_host.copy_(self.loss_dev, non_blocking=True)
+        self._fetch_host[0:1].copy_(self.loss_dev, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         return float(self._fetch_host[0])
 
@@ -458,7 +370,7 @@ class PolicyGradientsAgent(object):
         """the episode counter, the gradient accumulator, the per-timestep table, the noise schedule and every
         stream's cut position; the rows of episodes still open are not saved (a restore discards those episodes)"""
         torch.cuda.current_stream().synchronize()
-        state = {"segments": self.segments.state(), "current_episode": int(self.current_episode),
+        state = {"segments": super().checkpoint_state(), "current_episode": int(self.current_episode),
                  "training_iteration": int(self.training_iteration),
                  "accumulator": _pack(self.accumulator), "table": _pack(self.table)}
         if self.continuous:
@@ -466,7 +378,7 @@ class PolicyGradientsAgent(object):
         return state
 
     def restore_checkpoint_state(self, state):
-        self.segments.restore(state["segments"])
+        super().restore_checkpoint_state(state["segments"])
         sg = self.segments
         # an episode open at the checkpoint (or one that ended but was not trained yet) has rows the checkpoint does
         # not hold: it is neither learned nor counted

@@ -201,24 +201,35 @@ class QNetworkInstance(object):
                                                           _lib.current_stream()))
         return self.q
 
-    # ---- plain Q head computed by the agent's fused head kernel (cb200_dqn_head_fused) ------------------------------------
-    def head_fusable(self):
-        """plain Dense(num_actions) head on a 256- or 512-wide feature layer whose fp32 activations are kept"""
+    # ---- a head computed by one of the agents' fused head kernels --------------------------------------------------------
+    def feature_head(self):
+        """the head is one Dense on a 256- or 512-wide ReLU feature layer whose fp32 activations are kept: what every
+        fused head kernel reads"""
         if self.net.dueling or len(self.trunk.layers) < 2:
             return False
         head = self.trunk.layers[-1]
-        return (type(head).__name__ == "Dense" and head.K in (256, 512) and head.N <= 8 and
-                self.trunk.acts[-2] is not None and self.trunk.layers[-2].act == 1)
+        return (type(head).__name__ == "Dense" and head.K in (256, 512) and self.trunk.acts[-2] is not None and
+                self.trunk.layers[-2].act == 1)
+
+    def head_fusable(self):
+        """plain Dense(num_actions) head of <= 8 actions (cb200_dqn_head_fused)"""
+        return self.feature_head() and self.trunk.layers[-1].N <= 8
 
     def ensemble_fusable(self):
-        """head copies of <= 8 actions each on a 256- or 512-wide feature layer whose fp32 activations are kept
-        (cb200_ensemble_head_fused)"""
-        if self.net.dueling or len(self.trunk.layers) < 2:
-            return False
-        head = self.trunk.layers[-1]
-        return (type(head).__name__ == "Dense" and head.K in (256, 512) and self.net.num_actions <= 8 and
-                head.N == self.net.head_copies * self.net.num_actions and self.trunk.acts[-2] is not None and
-                self.trunk.layers[-2].act == 1)
+        """head copies of <= 8 actions each (cb200_ensemble_head_fused)"""
+        return (self.feature_head() and self.net.num_actions <= 8 and
+                self.trunk.layers[-1].N == self.net.head_copies * self.net.num_actions)
+
+    def bind_head_grads(self, d):
+        """points a fused head descriptor's gradient outputs at this training instance: dh (dL/d of the feature layer's
+        pre-activation, fp32 and / or its operand planes) and the head layer's dw / db in the gradient buffer"""
+        store = self.net.store
+        wname, bname = self.net.trunk.names[-1]
+        dz, pl = self.trunk.dzs[-2], self.trunk.dz_planes[-2]
+        d.dh = dz.data_ptr() if dz is not None else None
+        if pl is not None:
+            d.dh_planes, d.dh_plane_stride = pl.ptr, pl.stride
+        d.dw, d.db = store.view(store.grad, wname).data_ptr(), store.view(store.grad, bname).data_ptr()
 
     def forward_features(self):
         """everything below the head: the feature layer's post-ReLU output is ``features``"""

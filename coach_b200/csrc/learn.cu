@@ -830,6 +830,30 @@ __device__ __forceinline__ float ns_max(const float (&q)[kNsMaxA], int A) {
         if (a < A && (q[a] > m || q[a] != q[a])) m = q[a];
     return m;
 }
+// W [K, N] row-major -> Wt [N][K] in shared memory, by the whole block
+__device__ __forceinline__ void seg_head_wt(const float* __restrict__ w, int N, int K, float* wt) {
+    for (int i = threadIdx.x; i < N * K; i += blockDim.x) {
+        const int k = i / N, n = i - k * N;
+        wt[n * K + k] = __ldg(w + i);
+    }
+}
+// non-empty segments and the rows they cover (every warp counts them; integer sums are order-free)
+__device__ __forceinline__ void seg_count(const int32_t* __restrict__ seg_len, int S, int lane, int& nseg, int& used) {
+    nseg = 0;
+    used = 0;
+    for (int s = lane; s < S; s += 32) {
+        const int L = seg_len[s];
+        if (L > 0) {
+            nseg += 1;
+            used += L;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        nseg += __shfl_xor_sync(0xffffffffu, nseg, o);
+        used += __shfl_xor_sync(0xffffffffu, used, o);
+    }
+}
 
 template <int KPL>
 __global__ void __launch_bounds__(32 * kNsWarps, 1) nstep_q_head_kernel(NstepParams p) {
@@ -849,20 +873,8 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) nstep_q_head_kernel(NstepPar
         wt_tg[a * K + k] = __ldg(p.w_target + i);
     }
     for (int i = lane; i < A * K + 32; i += 32) dwacc[i] = 0.f;
-    // non-empty segments and the rows they cover (every warp counts them; integer sums are order-free)
-    int nseg = 0, used = 0;
-    for (int s = lane; s < p.S; s += 32) {
-        const int L = p.seg_len[s];
-        if (L > 0) {
-            nseg += 1;
-            used += L;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        nseg += __shfl_xor_sync(0xffffffffu, nseg, o);
-        used += __shfl_xor_sync(0xffffffffu, used, o);
-    }
+    int nseg, used;
+    seg_count(p.seg_len, p.S, lane, nseg, used);
     __syncthreads();
     const float w = nseg > 0 ? 1.0f / (float)nseg : 0.f;                 // the mean over segments
     float acc_loss = 0.f;
@@ -1086,24 +1098,10 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcP
     float* rowbuf = ac_smem + N * K + warp * (K + N * K + 32);
     float* dwacc = rowbuf + K;
     float* dbacc = dwacc + N * K;
-    for (int i = threadIdx.x; i < N * K; i += blockDim.x) {               // W [K, N] row-major -> Wt [N][K]
-        const int k = i / N, n = i - k * N;
-        wt[n * K + k] = __ldg(p.w + i);
-    }
+    seg_head_wt(p.w, N, K, wt);
     for (int i = lane; i < N * K + 32; i += 32) dwacc[i] = 0.f;
-    int nseg = 0, used = 0;
-    for (int s = lane; s < p.S; s += 32) {
-        const int L = p.seg_len[s];
-        if (L > 0) {
-            nseg += 1;
-            used += L;
-        }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        nseg += __shfl_xor_sync(0xffffffffu, nseg, o);
-        used += __shfl_xor_sync(0xffffffffu, used, o);
-    }
+    int nseg, used;
+    seg_count(p.seg_len, p.S, lane, nseg, used);
     __syncthreads();
     const float w = nseg > 0 ? 1.0f / (float)nseg : 0.f;                 // the mean over segments
     float acc_loss = 0.f;
@@ -1461,10 +1459,7 @@ __global__ void __launch_bounds__(32 * kPgWarps) pg_head_rows_kernel(PgParams p)
     float* rowbuf = pg_smem + N * K + warp * K;
     int* slot = reinterpret_cast<int*>(pg_smem + N * K + kPgWarps * K);
     const int r0 = blockIdx.x * kPgBlockRows;
-    for (int i = threadIdx.x; i < N * K; i += blockDim.x) {               // W [K, N] row-major -> Wt [N][K]
-        const int k = i / N, n = i - k * N;
-        wt[n * K + k] = __ldg(p.w + i);
-    }
+    seg_head_wt(p.w, N, K, wt);
     for (int j = threadIdx.x; j < kPgBlockRows; j += blockDim.x) slot[j] = -1;
     __syncthreads();
     for (int s = threadIdx.x; s < p.S; s += blockDim.x) {

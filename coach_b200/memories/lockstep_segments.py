@@ -2,9 +2,10 @@
 
   rl_coach/agents/policy_optimization_agent.py:85-135    segment cut every t_max steps or at the episode's end
 
-shared by the agents that learn from such segments (N-step Q, A3C, Policy Gradients).  Each stream behaves like one asynchronous reference
-worker: it has its own cut position and closes a segment when t_max (``num_steps_between_gradient_updates``) steps have
-passed since its last cut, or on game_over.  All segments closed at one lock-step are learned in ONE learn step.
+shared by the agents that learn from such segments: N-step Q, A3C and Policy Gradients, on the common agent base
+``coach_b200.agents.lockstep_agent``.  Each stream behaves like one asynchronous reference worker: it has its own cut
+position and closes a segment when t_max (``num_steps_between_gradient_updates``) steps have passed since its last
+cut, or on game_over.  All segments closed at one lock-step are learned in ONE learn step.
 
 Device rollout buffer: t_max slots per stream, slot (t mod t_max) * E + e for stream e at lock-step t: a segment spans at
 most t_max consecutive steps and is consumed at the step it closes, so a slot is never overwritten while it is live.

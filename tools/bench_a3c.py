@@ -52,7 +52,7 @@ def heads(agent):
     from coach_b200 import _lib
     st = _lib.current_stream()
     B = max(agent._buckets)
-    _, d, _ = agent._buckets[B]
+    d = agent._buckets[B].desc
     K, A, E = d.features, d.n_actions, agent.num_envs
     ac = time_call(lambda: agent.lib.cb200_actor_critic_head(ctypes.byref(d), st))
     z = lambda *s: torch.rand(*s, device="cuda")                                        # noqa: E731

@@ -88,7 +88,7 @@ def heads(agent):
     from coach_b200 import _lib
     st = _lib.current_stream()
     B = max(agent._buckets)
-    on, tn, d, _ = agent._buckets[B]
+    d = agent._buckets[B].desc
     K, A = d.features, d.n_actions
     ns = time_call(lambda: agent.lib.cb200_nstep_q_head(ctypes.byref(d), st))
     z = lambda *s: torch.rand(*s, device="cuda")                                        # noqa: E731

@@ -79,7 +79,7 @@ def kernels(agent):
     from coach_b200 import _lib
     st = _lib.current_stream()
     B = max(agent._buckets)
-    _, d, _ = agent._buckets[B]
+    d = agent._buckets[B].desc
     head = time_call(lambda: agent.lib.cb200_policy_gradient_head(ctypes.byref(d), st))
     off, ln = agent.segments.seg_table()
     tg = time_call(lambda: agent.lib.cb200_pg_targets(agent.returns.data_ptr(), off, ln, agent.num_envs, B,
