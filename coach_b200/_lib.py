@@ -132,6 +132,25 @@ class ActorCriticHeadDesc(ctypes.Structure):
 AC_A_VALUE, AC_GAE, AC_GAE_VALUE = 0, 1, 2
 
 
+class ActorCriticGaussianHeadDesc(ctypes.Structure):
+    """struct cb200_actor_critic_gaussian_head_desc"""
+    _fields_ = [("h", c_void_p), ("h_boot", c_void_p), ("w", c_void_p), ("b", c_void_p), ("actions", c_void_p),
+                ("max_abs_range", c_void_p), ("rewards", c_void_p), ("game_overs", c_void_p),
+                ("seg_offsets", c_void_p), ("seg_lengths", c_void_p), ("segments", ctypes.c_int32), ("rows", c_i64),
+                ("discount", c_double), ("gae_lambda", c_double), ("mode", ctypes.c_int32),
+                ("huber", ctypes.c_int32), ("beta_entropy", c_float), ("v_weight", c_float), ("p_weight", c_float),
+                ("features", ctypes.c_int32), ("action_dim", ctypes.c_int32), ("z", c_void_p), ("dz", c_void_p),
+                ("loss", c_void_p), ("means", c_void_p), ("stds", c_void_p), ("targets", c_void_p),
+                ("advantages", c_void_p), ("bootstrap", c_void_p), ("dh", c_void_p), ("dh_planes", c_void_p),
+                ("dh_plane_stride", c_i64), ("dw", c_void_p), ("db", c_void_p), ("workspace", c_void_p)]
+
+
+def acg_workspace_floats(rows, segments, features, action_dim):
+    """the floats cb200_actor_critic_gaussian_head's workspace takes"""
+    N, chunks = 1 + 2 * action_dim, (rows + 63) // 64
+    return rows * (N + 4) + segments + chunks * (features * N + N + 1)
+
+
 class PolicyGradientHeadDesc(ctypes.Structure):
     """struct cb200_policy_gradient_head_desc"""
     _fields_ = [("h", c_void_p), ("w", c_void_p), ("b", c_void_p), ("targets", c_void_p), ("actions", c_void_p),
@@ -203,6 +222,9 @@ PROTOTYPES = {
     "cb200_ensemble_head_fused": (c_int, [c_void_p, c_void_p]),
     "cb200_nstep_q_head": (c_int, [c_void_p, c_void_p]),
     "cb200_actor_critic_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_actor_critic_gaussian_head": (c_int, [c_void_p, c_void_p]),
+    "cb200_gaussian_policy_act": (c_int, [c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p]),
     "cb200_categorical_act": (c_int, [c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "cb200_pg_targets": (c_int, [c_void_p, c_void_p, c_void_p, ctypes.c_int32, c_i64, ctypes.c_int32, c_void_p,
                                  c_void_p, ctypes.c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),

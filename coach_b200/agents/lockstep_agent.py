@@ -27,9 +27,10 @@ class LockstepAgent(object):
     is_on_policy = True
 
     def __init__(self, ap, parent, observation_shape, num_envs, device, seed, outputs, value_head=False,
-                 action_dim=None):
+                 action_dim=None, gaussian_policy=False, depth=None):
         """the constructor's common part; the subclass validates its parameters first.  outputs: the head's policy or
-        Q outputs (value_head adds V's column); action_dim: float action vectors of that width (continuous actions)"""
+        Q outputs (value_head adds V's column; gaussian_policy: they are a mean and a std block); action_dim: float
+        action vectors of that width (continuous actions); depth: the rollout ring's rows per stream (default t_max)"""
         net_params = ap.network_wrappers["main"]
         self.ap, self.parent = ap, parent
         self.lib = _lib.load()
@@ -42,10 +43,10 @@ class LockstepAgent(object):
         scheme = getattr(getattr(net_params, "middleware_parameters", None), "scheme", "Medium")
         self.net_def = QNetworkDef(dev, obs, outputs, middleware_units=middleware_units(scheme),
                                    embedder_scheme=scheme_layers(getattr(emb, "scheme", "Medium")),
-                                   value_head=value_head)
+                                   value_head=value_head, gaussian_policy=gaussian_policy)
         gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
         self.net_def.store.init_glorot(gen)
-        self.segments = sg = LockstepSegments(self.lib, dev, obs, E, self.t_max, action_dim)
+        self.segments = sg = LockstepSegments(self.lib, dev, obs, E, self.t_max, action_dim, depth)
         self.learn = sg.learn
         # the shared parameters (online, target, Adam) and the acting path of the DQN agent.  The wrapper's own
         # bindings are the 32-row bucket.

@@ -48,8 +48,8 @@ from coach_b200 import _lib, parallel
 from coach_b200.agents.actor_critic_agent import CategoricalParameters, PolicyGradientRescaler
 from coach_b200.agents.lockstep_agent import LockstepAgent
 from coach_b200.base_parameters import AgentParameters, AlgorithmParameters, InputEmbedderParameters, NetworkParameters
-from coach_b200.memories.lockstep_segments import round32
-from coach_b200.schedules import LinearSchedule
+from coach_b200.exploration_policies.additive_noise import AdditiveNoiseParameters
+from coach_b200.memories.lockstep_segments import bucket_rows
 
 __all__ = ["PolicyGradientRescaler", "PolicyGradientAlgorithmParameters", "PolicyGradientNetworkParameters",
            "AdditiveNoiseParameters", "PolicyGradientsAgentParameters", "PolicyGradientsAgent"]
@@ -77,19 +77,6 @@ class PolicyGradientNetworkParameters(NetworkParameters):
         self.async_training = True
 
 
-class AdditiveNoiseParameters(object):
-    """exploration_policies/additive_noise.py:29-39"""
-
-    def __init__(self):
-        self.noise_schedule = LinearSchedule(0.1, 0.1, 50000)
-        self.evaluation_noise = 0.05
-        self.noise_as_percentage_from_action_space = True
-
-    @property
-    def path(self):
-        return 'rl_coach.exploration_policies.additive_noise:AdditiveNoise'
-
-
 class PolicyGradientsAgentParameters(AgentParameters):
     """policy_gradients_agent.py:68-79; the reference's SingleEpisodeBuffer is the agent's device rollout buffer"""
 
@@ -108,16 +95,6 @@ RESCALERS = {PolicyGradientRescaler.TOTAL_RETURN: _lib.PG_TOTAL_RETURN,
              PolicyGradientRescaler.FUTURE_RETURN: _lib.PG_FUTURE_RETURN,
              PolicyGradientRescaler.FUTURE_RETURN_NORMALIZED_BY_EPISODE: _lib.PG_NORMALIZED_BY_EPISODE,
              PolicyGradientRescaler.FUTURE_RETURN_NORMALIZED_BY_TIMESTEP: _lib.PG_NORMALIZED_BY_TIMESTEP}
-
-
-def bucket_rows(n):
-    """the learn step's row bucket for n rows: n rounded up to 32 up to 256 rows, above that to a quarter of the power of
-    two below n (256 -> 320 -> 384 -> 448 -> 512 -> 640 -> ...)"""
-    n = round32(n)
-    if n <= 256:
-        return n
-    step = 1 << ((n - 1).bit_length() - 3)
-    return -(-n // step) * step
 
 
 def _pack(t):

@@ -27,7 +27,7 @@ class ParamStore(object):
         self.theta = None
         self.glorot_fans = {}             # kernel name -> (fan_in, fan_out) when it is not the tensor's own
         self.initial_values = {}          # rescaler name -> initial value (default 1.0)
-        self.normalized_columns = {}      # kernel name -> (first n columns, std): normalized_columns_initializer
+        self.normalized_columns = {}      # kernel name -> [(first column, columns, std)]: normalized_columns_initializer
 
     def add(self, name, shape):
         if self.theta is not None:
@@ -70,10 +70,9 @@ class ParamStore(object):
                 fan_in, fan_out = self.glorot_fans.get(name, (fan_in, fan_out))
                 limit = float(np.sqrt(6.0 / (fan_in + fan_out)))
                 cpu = (torch.rand(shape, generator=generator, dtype=torch.float32) * 2 - 1) * limit
-                if name in self.normalized_columns:          # head.py:28-33: randn scaled to a column norm of std
-                    n, std = self.normalized_columns[name]
-                    w = torch.randn((shape[0], n), generator=generator, dtype=torch.float32)
-                    cpu[:, :n] = w * (std / torch.sqrt((w * w).sum(dim=0, keepdim=True)))
+                for c0, n, std in self.normalized_columns.get(name, ()):   # head.py:28-33: randn scaled to a column
+                    w = torch.randn((shape[0], n), generator=generator, dtype=torch.float32)    # norm of std
+                    cpu[:, c0:c0 + n] = w * (std / torch.sqrt((w * w).sum(dim=0, keepdim=True)))
                 v.copy_(cpu)
             elif name.endswith("rescalers"):
                 v.fill_(self.initial_values.get(name, 1.0))

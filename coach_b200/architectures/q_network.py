@@ -27,7 +27,7 @@ class QNetworkDef(object):
     """Parameter layout + layer chain; instances bind it to buffers (see QNetworkInstance)."""
 
     def __init__(self, device, observation_shape, num_actions, dueling=False, embedder="auto", middleware_units=512,
-                 head_copies=1, head_grad_rescale=1.0, embedder_scheme=None, value_head=False):
+                 head_copies=1, head_grad_rescale=1.0, embedder_scheme=None, value_head=False, gaussian_policy=False):
         """embedder_scheme: the input embedder's layers (InputEmbedderParameters.scheme as a list): for images a list of
         base_parameters.Conv2d specs, for vectors a list of base_parameters.Dense specs; None is the Medium embedder
         above (image_embedder.py:62-67 / vector_embedder.py:58-61).
@@ -40,8 +40,14 @@ class QNetworkDef(object):
         value_head (ActorCritic): VHead Dense(1) + PolicyHead Dense(num_actions) as ONE Dense(1 + num_actions); column 0
         is initialised as normalized_columns_initializer(1.0) (v_head.py:44-47, head.py:28-33), the policy block
         Glorot-uniform with the fans of its own [F, num_actions] layer; one ``gradients_from_head_{0,1}-0_rescalers``
-        scalar per head."""
+        scalar per head.
+        gaussian_policy (with value_head, continuous actions; policy_head.py:102-152 with ContinuousEntropy): the
+        num_actions = 2 D policy columns are fc_mean (columns 1..D, Glorot-uniform with the fans of its own [F, D]
+        layer) and fc_std (columns D+1..2D, normalized_columns_initializer(0.01))."""
         self.value_head = bool(value_head)
+        self.gaussian_policy = bool(gaussian_policy)
+        if self.gaussian_policy and not (self.value_head and num_actions % 2 == 0):
+            raise ValueError("gaussian_policy takes value_head and an even number of policy columns (mean | std)")
         if self.value_head and (dueling or head_copies != 1):
             raise NotImplementedError("the actor-critic head takes neither a dueling head nor head copies")
         self.head_copies = int(head_copies)
@@ -82,10 +88,15 @@ class QNetworkDef(object):
             layers.append(Dense(middleware_units, self.head_copies * self.num_actions + self.value_head, None))
             self.trunk = Sequential(layers, self.store, "main/online/network_0")
             self.v_tower = self.a_tower = None
-            if self.head_copies > 1 or self.value_head:
-                self.store.glorot_fans[self.trunk.names[-1][0]] = (middleware_units, self.num_actions)
-            if self.value_head:
-                self.store.normalized_columns[self.trunk.names[-1][0]] = (1, 1.0)
+            kernel = self.trunk.names[-1][0]
+            if self.gaussian_policy:
+                D = self.num_actions // 2
+                self.store.glorot_fans[kernel] = (middleware_units, D)
+                self.store.normalized_columns[kernel] = [(0, 1, 1.0), (1 + D, D, 0.01)]
+            elif self.head_copies > 1 or self.value_head:
+                self.store.glorot_fans[kernel] = (middleware_units, self.num_actions)
+            if self.value_head and not self.gaussian_policy:
+                self.store.normalized_columns[kernel] = [(0, 1, 1.0)]
         else:
             self.trunk = Sequential(layers, self.store, "main/online/network_0")
             self.v_tower = Sequential([Dense(middleware_units, 512, "relu"), Dense(512, 1, None)], self.store,

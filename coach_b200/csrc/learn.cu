@@ -1039,6 +1039,30 @@ __device__ __forceinline__ double ac_lfilter(double x, double& z, double c) {
     return y;
 }
 
+// One row i (walking i = L-1 .. 0) of a segment's backward recurrence (actor_critic_agent.py:111-150), shared by the
+// discrete and the Gaussian heads: given the row's reward rw and V, the fp64 target and advantage in numpy's /
+// scipy.signal.lfilter's operation order.  The state: vnext (V of the next row; first the bootstrap value, 0 after a
+// terminal state), A_VALUE's R and boot_pending (true until the first step of a bootstrapped segment), GAE's filter
+// delays za / zr (zr started with ac_lfilter(vnext, zr, gamma)); gl = discount * gae_lambda, gamma32 = (float) discount.
+__device__ __forceinline__ void ac_recurrence_step(int mode, double rw, float v, double gamma, float gamma32, double gl,
+                                                   float& vnext, double& R, bool& boot_pending, double& za, double& zr,
+                                                   double& target, double& adv) {
+    if (mode == CB200_AC_A_VALUE) {
+        // R = r_i + discount * R; right after a bootstrap, python float * np.float32 is an fp32 product
+        R = boot_pending ? __dadd_rn(rw, (double)__fmul_rn(gamma32, vnext)) : __dadd_rn(rw, __dmul_rn(gamma, R));
+        boot_pending = false;
+        target = R;
+        adv = __dsub_rn(R, (double)v);
+    } else {
+        // deltas = rewards + discount * values[1:] - values[:-1]: every discount * value is an fp32 product
+        const double delta = __dsub_rn(__dadd_rn(rw, (double)__fmul_rn(gamma32, vnext)), (double)v);
+        adv = ac_lfilter(delta, za, gl);
+        const double ret = ac_lfilter(rw, zr, gamma);
+        target = mode == CB200_AC_GAE_VALUE ? __dadd_rn(adv, (double)v) : ret;
+    }
+    vnext = v;
+}
+
 // PolicyHead's discrete terms of one row (heads/policy_head.py:91-100), shared by the actor-critic and the policy
 // gradient heads: p = softmax(logits z[1..A]); Categorical(probs = p + eps): ls = log_softmax(log(p + eps)) (probs not
 // renormalised), H = -sum u ls, logp = ls[act] (0 for an action outside [0, A)), u_act = p[act] + eps, su = sum u.
@@ -1132,20 +1156,7 @@ __global__ void __launch_bounds__(32 * kNsWarps, 1) actor_critic_head_kernel(AcP
             ns_dot<KPL, kAcMaxN>(p.h + (size_t)r * K, wt, p.b, N, K, lane, hv, z);     // hv = this row's features
             const float v = z[0];
             double target, adv;
-            if (p.mode == CB200_AC_A_VALUE) {
-                // R = r_i + discount * R; right after a bootstrap, python float * np.float32 is an fp32 product
-                R = boot_pending ? __dadd_rn(rw, (double)__fmul_rn(gamma32, vnext)) : __dadd_rn(rw, __dmul_rn(gamma, R));
-                boot_pending = false;
-                target = R;
-                adv = __dsub_rn(R, (double)v);
-            } else {
-                // deltas = rewards + discount * values[1:] - values[:-1]: every discount * value is an fp32 product
-                const double delta = __dsub_rn(__dadd_rn(rw, (double)__fmul_rn(gamma32, vnext)), (double)v);
-                adv = ac_lfilter(delta, za, gl);
-                const double ret = ac_lfilter(rw, zr, gamma);
-                target = p.mode == CB200_AC_GAE_VALUE ? __dadd_rn(adv, (double)v) : ret;
-            }
-            vnext = v;
+            ac_recurrence_step(p.mode, rw, v, gamma, gamma32, gl, vnext, R, boot_pending, za, zr, target, adv);
             const float t32 = (float)target, a32 = (float)adv;
             // policy: p = softmax(logits); Categorical(probs = p + eps): log_softmax(log(p + eps)), probs not renormalised
             float pr[kNsMaxA], ls[kNsMaxA], ent, logp, u_act, su;
@@ -1585,6 +1596,230 @@ __global__ void pg_gaussian_act_kernel(const float* __restrict__ z, int64_t envs
     const float mu = pg_mean(z[i], range[d], th);
     actions[i] = normals ? __dadd_rn((double)mu, __dmul_rn(scale[i], normals[i])) : (double)mu;
     if (means) means[i] = mu;
+}
+
+// ---- actor-critic (A3C) head, continuous actions ----------------------------------------------------------------------
+// ONE Dense(1 + 2D) on the feature layer: column 0 V, columns 1..D the pre-tanh means, D+1..2D the pre-softplus stds
+// (policy_head.py:102-152 with ContinuousEntropy).  Segments are whole episodes (up to 1000 rows and more), so the head
+// is parallel over rows, not over segments:
+//   ac_gauss_rows_kernel      Z = hW + b of every row and each segment's bootstrap V(s'_last); every row's slot = -1
+//   ac_gauss_segments_kernel  one thread per segment: the fp64 recurrence of the discrete head (AcRecurrence) on Z[:, 0]
+//                             -> targets, advantages and the rows' segment slot
+//   ac_gauss_grad_kernel      per row the three loss terms, dL/dZ over the 1 + 2D columns and dL/dh; rows no segment
+//                             covers get zero outputs
+// then pg_head_dw_kernel and dqn_head_reduce_kernel sum dW, db and the loss per 64-row chunk and over the chunks in a
+// fixed order.
+constexpr int kAcgMaxD = 17;                                              // Humanoid: every mujoco_v2 level
+constexpr int kAcgMaxN = 1 + 2 * kAcgMaxD;
+
+struct AcGaussParams {
+    const float *h, *h_boot, *w, *b, *actions, *range;
+    const double* rewards;
+    const uint8_t* game_overs;
+    const int32_t *seg_off, *seg_len;
+    int S, rows, mode, huber, K, D, N;
+    double discount, gae_lambda;
+    float beta_entropy, v_weight, p_weight;
+    float *z, *dz, *targets, *advantages, *bootstrap, *means, *stds, *rowloss, *dh;
+    int32_t* row_seg;
+    uint16_t* dh_planes;
+    int64_t dh_plane_stride;
+};
+
+// softplus(x) + eps with TF 1.x's softplus (the Eigen functor): x above -threshold, exp(x) below threshold,
+// log(exp(x) + 1) between, threshold = log(FLT_EPSILON) + 2; eps = np.finfo(np.float32).eps
+__device__ __forceinline__ float acg_std(float x) {
+    const float eps = 1.1920928955078125e-07f;
+    const float threshold = logf(eps) + 2.0f;
+    const float e = expf(x);
+    const float sp = x > -threshold ? x : (x < threshold ? e : logf(e + 1.0f));
+    return sp + eps;
+}
+
+// rows [0, rows) and then the S bootstrap rows, kPgBlockRows per block, kPgWarpRows per warp
+template <int KPL>
+__global__ void __launch_bounds__(32 * kPgWarps) ac_gauss_rows_kernel(AcGaussParams p) {
+    extern __shared__ __align__(16) float acg_smem[];                     // Wt [N][K]
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int N = p.N, K = p.K;
+    float* wt = acg_smem;
+    seg_head_wt(p.w, N, K, wt);
+    __syncthreads();
+    for (int rr = 0; rr < kPgWarpRows; ++rr) {
+        const int r = blockIdx.x * kPgBlockRows + warp * kPgWarpRows + rr;
+        float hv[KPL], z[kAcgMaxN];
+        if (r < p.rows) {
+            ns_dot<KPL, kAcgMaxN>(p.h + (size_t)r * K, wt, p.b, N, K, lane, hv, z);
+            if (lane == 0) {
+#pragma unroll
+                for (int n = 0; n < kAcgMaxN; ++n)
+                    if (n < N) p.z[(size_t)r * N + n] = z[n];
+                p.row_seg[r] = -1;
+            }
+        } else if (r < p.rows + p.S) {
+            // V(s'_last) of the online network, 0 after a terminal state or for an unused slot
+            const int s = r - p.rows, L = p.seg_len[s], o = p.seg_off[s];
+            const bool valid = L > 0 && o >= 0 && (int64_t)o + L <= p.rows;
+            float vnext = 0.f;
+            if (valid && !p.game_overs[o + L - 1]) {
+                ns_dot<KPL, kAcgMaxN>(p.h_boot + (size_t)s * K, wt, p.b, 1, K, lane, hv, z);
+                vnext = z[0];
+            }
+            if (lane == 0) p.bootstrap[s] = vnext;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(128) ac_gauss_segments_kernel(AcGaussParams p) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= p.S) return;
+    const int L = p.seg_len[s], o = p.seg_off[s];
+    if (!(L > 0 && o >= 0 && (int64_t)o + L <= p.rows)) return;
+    // the discrete head's state and start (actor_critic_head_kernel)
+    float vnext = p.bootstrap[s];
+    const double gamma = p.discount, gl = __dmul_rn(p.discount, p.gae_lambda);
+    const float gamma32 = (float)p.discount;
+    double R = 0.0, za = 0.0, zr = 0.0;
+    bool boot_pending = !p.game_overs[o + L - 1];
+    if (p.mode != CB200_AC_A_VALUE) ac_lfilter((double)vnext, zr, gamma);
+    for (int i = L - 1; i >= 0; --i) {
+        const int r = o + i;
+        double target, adv;
+        ac_recurrence_step(p.mode, p.rewards[r], p.z[(size_t)r * p.N], gamma, gamma32, gl, vnext, R, boot_pending, za,
+                           zr, target, adv);
+        p.targets[r] = (float)target;
+        p.advantages[r] = (float)adv;
+        p.row_seg[r] = s;
+    }
+}
+
+template <int KPL>
+__global__ void __launch_bounds__(32 * kPgWarps) ac_gauss_grad_kernel(AcGaussParams p) {
+    // Wt [N][K] | row buffers [warps][K]
+    extern __shared__ __align__(16) float acg_smem[];
+    __shared__ int nseg_shared;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int N = p.N, K = p.K, D = p.D;
+    float* wt = acg_smem;
+    float* rowbuf = acg_smem + N * K + warp * K;
+    if (threadIdx.x == 0) nseg_shared = 0;
+    seg_head_wt(p.w, N, K, wt);
+    __syncthreads();
+    int mine = 0;                                                         // non-empty segments (order-free integer sum)
+    for (int s = threadIdx.x; s < p.S; s += blockDim.x) mine += p.seg_len[s] > 0 ? 1 : 0;
+    if (mine) atomicAdd(&nseg_shared, mine);
+    __syncthreads();
+    const int nseg = nseg_shared;
+    const float w = nseg > 0 ? 1.0f / (float)nseg : 0.f;                 // the mean over segments
+    const float log2pi = 1.8378770664093453f;
+    for (int rr = 0; rr < kPgWarpRows; ++rr) {
+        const int r = blockIdx.x * kPgBlockRows + warp * kPgWarpRows + rr;
+        if (r >= p.rows) break;
+        const int s = p.row_seg[r];
+        // dL/dZ of V, of the mean block and of the std block (indexed by d only, so they stay in registers)
+        float hv[KPL], dz0 = 0.f, dzm[kAcgMaxD], dzs[kAcgMaxD];
+        float row_loss = 0.f;
+#pragma unroll
+        for (int d = 0; d < kAcgMaxD; ++d) dzm[d] = dzs[d] = 0.f;
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) hv[j] = s >= 0 ? __ldg(p.h + (size_t)r * K + lane + 32 * j) : 0.f;
+        if (s >= 0) {
+            const float c = w * (1.0f / (float)p.seg_len[s]);            // the row weight 1 / (segments L)
+            const float* zr = p.z + (size_t)r * N;
+            const float v = zr[0], t32 = p.targets[r], a32 = p.advantages[r];
+            const float e = v - t32;
+            float lv, gv;
+            if (p.huber) {
+                const float ae = fabsf(e);
+                const float qq = fminf(ae, 1.0f);
+                lv = 0.5f * qq * qq + (ae - qq);
+                gv = fmaxf(-1.0f, fminf(e, 1.0f));
+            } else {
+                lv = e * e;
+                gv = 2.0f * e;
+            }
+            dz0 = c * p.v_weight * gv;
+            // MultivariateNormalDiag(mean, std): log pi = sum_d -((x - mean) / std)^2 / 2 - log std - log(2 pi) / 2,
+            // H = sum_d (1 + log(2 pi)) / 2 + log std
+            const float cp = -c * p.p_weight * a32, cb = c * p.beta_entropy;
+            float logp = 0.f, ent = 0.f;
+#pragma unroll
+            for (int d = 0; d < kAcgMaxD; ++d)
+                if (d < D) {
+                    const float rg = __ldg(p.range + d);
+                    float th;
+                    const float mu = pg_mean(zr[1 + d], rg, th);
+                    const float zs = zr[1 + D + d];
+                    const float sd = acg_std(zs);
+                    const float diff = p.actions[(size_t)r * D + d] - mu;
+                    const float y = diff / sd, lsd = logf(sd);
+                    logp += -0.5f * y * y - lsd - 0.5f * log2pi;
+                    ent += 0.5f * (1.0f + log2pi) + lsd;
+                    dzm[d] = cp * (diff / (sd * sd)) * rg * (1.0f - th * th);
+                    const float sig = 1.0f / (expf(-zs) + 1.0f);          // TF's SoftplusGrad: dy / (exp(-x) + 1)
+                    dzs[d] = (cp * (diff * diff / (sd * sd * sd) - 1.0f / sd) - cb / sd) * sig;
+                    if (lane == 0) {
+                        if (p.means) p.means[(size_t)r * D + d] = mu;
+                        if (p.stds) p.stds[(size_t)r * D + d] = sd;
+                    }
+                }
+            row_loss = c * (p.v_weight * lv - p.p_weight * logp * a32 - p.beta_entropy * ent);
+        }
+        if (lane == 0) {
+            float* dzr = p.dz + (size_t)r * N;
+            dzr[0] = dz0;
+#pragma unroll
+            for (int d = 0; d < kAcgMaxD; ++d)
+                if (d < D) {
+                    dzr[1 + d] = dzm[d];
+                    dzr[1 + D + d] = dzs[d];
+                }
+            if (s < 0) {
+                for (int n = 0; n < N; ++n) p.z[(size_t)r * N + n] = 0.f;
+                p.targets[r] = 0.f;
+                p.advantages[r] = 0.f;
+                for (int d = 0; d < D; ++d) {
+                    if (p.means) p.means[(size_t)r * D + d] = 0.f;
+                    if (p.stds) p.stds[(size_t)r * D + d] = 0.f;
+                }
+            }
+            p.rowloss[r] = row_loss;
+        }
+        __syncwarp();                                                     // the previous row's readers are done
+#pragma unroll
+        for (int j = 0; j < KPL; ++j) {
+            const int k = lane + 32 * j;
+            float sdh = dz0 * wt[k];                                      // the columns in order
+#pragma unroll
+            for (int d = 0; d < kAcgMaxD; ++d)
+                if (d < D) sdh = fmaf(dzm[d], wt[(1 + d) * K + k], sdh);
+#pragma unroll
+            for (int d = 0; d < kAcgMaxD; ++d)
+                if (d < D) sdh = fmaf(dzs[d], wt[(1 + D + d) * K + k], sdh);
+            rowbuf[k] = hv[j] > 0.f ? sdh : 0.f;                          // relu'(h) on the post-activation value
+        }
+        __syncwarp();
+        head_store_dz<KPL>(rowbuf, lane, r, K, p.dh, p.dh_planes, p.dh_plane_stride);
+    }
+}
+
+// acting of the continuous actor-critic head: thread per (environment, dimension) on z [envs, 1 + 2D]: the head's
+// mean tanh(z) * range and std softplus(z) + eps (fp32), then numpy's normal(mean, std) = mean + std * n in fp64 on
+// host standard normals, or the mean
+__global__ void ac_gauss_act_kernel(const float* __restrict__ z, int64_t envs, int D, const float* __restrict__ range,
+                                    const double* __restrict__ normals, double* __restrict__ actions,
+                                    float* __restrict__ means, float* __restrict__ stds) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= envs * D) return;
+    const int64_t e = i / D;
+    const int d = (int)(i - e * D);
+    const float* ze = z + e * (1 + 2 * D);
+    float th;
+    const float mu = pg_mean(ze[1 + d], range[d], th);
+    const float sd = acg_std(ze[1 + D + d]);
+    actions[i] = normals ? __dadd_rn((double)mu, __dmul_rn((double)sd, normals[i])) : (double)mu;
+    if (means) means[i] = mu;
+    if (stds) stds[i] = sd;
 }
 
 }  // namespace cb200
@@ -2039,6 +2274,89 @@ int cb200_policy_act(const float* z, int64_t envs, int32_t n_outputs, int32_t co
         CB200_LAUNCH(pg_gaussian_act_kernel, (unsigned)((n + 127) / 128), 128, 0, st, z, envs, n_outputs, max_abs_range,
                      draws, scale, cont_actions, means);
     }
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_actor_critic_gaussian_head(const cb200_actor_critic_gaussian_head_desc* d, void* stream) {
+    CB200_CHECK_ARG(d != nullptr, "null descriptor");
+    CB200_CHECK_ARG(d->mode >= CB200_AC_A_VALUE && d->mode <= CB200_AC_GAE_VALUE, "unknown mode");
+    CB200_CHECK_ARG(d->h && d->h_boot && d->w && d->b && d->actions && d->max_abs_range && d->rewards &&
+                        d->game_overs && d->seg_offsets && d->seg_lengths && d->z && d->dw && d->db && d->workspace,
+                    "null pointer");
+    CB200_CHECK_ARG(d->segments >= 1 && d->segments <= (1 << 20), "1 <= segments <= 2^20");
+    CB200_CHECK_ARG(d->rows >= 1 && d->rows <= (1 << 24), "1 <= rows <= 2^24");
+    CB200_CHECK_ARG(d->action_dim >= 1 && d->action_dim <= kAcgMaxD, "1 <= action_dim <= 17");
+    CB200_CHECK_ARG(d->features == 256 || d->features == 512, "features must be 256 or 512");
+    CB200_CHECK_ARG(!d->dh_planes || (d->dh_plane_stride % 8 == 0 && d->rows % 8 == 0), "planes: rows % 8, stride % 8");
+    const int rows = (int)d->rows, K = d->features, D = d->action_dim, N = 1 + 2 * D, S = d->segments;
+    AcGaussParams p;
+    p.h = d->h; p.h_boot = d->h_boot; p.w = d->w; p.b = d->b; p.actions = d->actions; p.range = d->max_abs_range;
+    p.rewards = d->rewards; p.game_overs = d->game_overs; p.seg_off = d->seg_offsets; p.seg_len = d->seg_lengths;
+    p.S = S; p.rows = rows; p.mode = d->mode; p.huber = d->huber; p.K = K; p.D = D; p.N = N;
+    p.discount = d->discount; p.gae_lambda = d->gae_lambda;
+    p.beta_entropy = d->beta_entropy; p.v_weight = d->v_weight; p.p_weight = d->p_weight;
+    p.z = d->z; p.means = d->means; p.stds = d->stds; p.dh = d->dh;
+    p.dh_planes = static_cast<uint16_t*>(d->dh_planes); p.dh_plane_stride = d->dh_plane_stride;
+    // workspace: dL/dZ [rows, N] | per-row losses | targets | advantages | row slots [rows] | bootstrap [segments] |
+    // chunk partials; the optional outputs replace their workspace slices
+    float* ws = d->workspace;
+    p.dz = d->dz ? d->dz : ws;
+    p.rowloss = ws + (size_t)rows * N;
+    p.targets = d->targets ? d->targets : p.rowloss + rows;
+    p.advantages = d->advantages ? d->advantages : p.rowloss + 2 * (size_t)rows;
+    p.row_seg = reinterpret_cast<int32_t*>(p.rowloss + 3 * (size_t)rows);
+    p.bootstrap = d->bootstrap ? d->bootstrap : p.rowloss + 4 * (size_t)rows;
+    float* part = p.rowloss + 4 * (size_t)rows + S;
+    cudaStream_t st = as_stream(stream);
+    // up to 78 KB at K = 512, N = 35 (the staged kernel and eight row buffers): opted into once per instantiation and
+    // device, at the size of the largest shape
+    auto smem_of = [](int N, int K) { return (size_t)(N * K + kPgWarps * K) * sizeof(float); };
+    static bool attr_set[kMaxDevices][2] = {};
+    int dev = 0;
+    CB200_CUDA(cudaGetDevice(&dev));
+    CB200_CHECK_ARG(dev < kMaxDevices, "device ordinal out of range");
+    const int ti = K == 512 ? 1 : 0;
+    if (!attr_set[dev][ti]) {
+        const int most = (int)smem_of(kAcgMaxN, K);
+        if (ti) {
+            CB200_CUDA(cudaFuncSetAttribute(ac_gauss_rows_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+            CB200_CUDA(cudaFuncSetAttribute(ac_gauss_grad_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+        } else {
+            CB200_CUDA(cudaFuncSetAttribute(ac_gauss_rows_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+            CB200_CUDA(cudaFuncSetAttribute(ac_gauss_grad_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, most));
+        }
+        attr_set[dev][ti] = true;
+    }
+    const unsigned row_grid = (unsigned)((rows + S + kPgBlockRows - 1) / kPgBlockRows);
+    const unsigned grad_grid = (unsigned)((rows + kPgBlockRows - 1) / kPgBlockRows);
+    const size_t smem_rows = (size_t)N * K * sizeof(float), smem_grad = smem_of(N, K);
+    if (K == 512) {
+        CB200_LAUNCH(ac_gauss_rows_kernel<16>, row_grid, 32 * kPgWarps, smem_rows, st, p);
+        CB200_LAUNCH(ac_gauss_segments_kernel, (unsigned)((S + 127) / 128), 128, 0, st, p);
+        CB200_LAUNCH(ac_gauss_grad_kernel<16>, grad_grid, 32 * kPgWarps, smem_grad, st, p);
+    } else {
+        CB200_LAUNCH(ac_gauss_rows_kernel<8>, row_grid, 32 * kPgWarps, smem_rows, st, p);
+        CB200_LAUNCH(ac_gauss_segments_kernel, (unsigned)((S + 127) / 128), 128, 0, st, p);
+        CB200_LAUNCH(ac_gauss_grad_kernel<8>, grad_grid, 32 * kPgWarps, smem_grad, st, p);
+    }
+    const int n_out = K * N + N + 1, chunks = (rows + kPgChunk - 1) / kPgChunk;
+    const dim3 dw_grid((unsigned)((n_out + 255) / 256), (unsigned)min(chunks, 65535));
+    CB200_LAUNCH(pg_head_dw_kernel, dw_grid, 256, 0, st, d->h, p.dz, p.rowloss, rows, K, N, part);
+    CB200_LAUNCH(dqn_head_reduce_kernel, (unsigned)((n_out + 31) / 32), 256, 0, st, part, chunks, n_out, K * N, N, 1.0f,
+                 d->dw, d->db, d->loss);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_gaussian_policy_act(const float* z, int64_t envs, int32_t action_dim, const float* max_abs_range,
+                              const double* normals, double* actions, float* means, float* stds, void* stream) {
+    CB200_CHECK_ARG(z && max_abs_range && actions, "null pointer");
+    CB200_CHECK_ARG(envs >= 1 && envs <= (1 << 24), "1 <= envs <= 2^24");
+    CB200_CHECK_ARG(action_dim >= 1 && action_dim <= kAcgMaxD, "1 <= action_dim <= 17");
+    const int64_t n = envs * action_dim;
+    CB200_LAUNCH(ac_gauss_act_kernel, (unsigned)((n + 127) / 128), 128, 0, as_stream(stream), z, envs, action_dim,
+                 max_abs_range, normals, actions, means, stds);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

@@ -7,8 +7,11 @@ shared by the agents that learn from such segments: N-step Q, A3C and Policy Gra
 position and closes a segment when t_max (``num_steps_between_gradient_updates``) steps have passed since its last
 cut, or on game_over.  All segments closed at one lock-step are learned in ONE learn step.
 
-Device rollout buffer: t_max slots per stream, slot (t mod t_max) * E + e for stream e at lock-step t: a segment spans at
-most t_max consecutive steps and is consumed at the step it closes, so a slot is never overwritten while it is live.
+Device rollout buffer: ``depth`` slots per stream (default t_max), slot (t mod depth) * E + e for stream e at lock-step
+t: a segment spans at most t_max consecutive steps and is consumed at the step it closes, so with depth = t_max a slot is
+never overwritten while it is live.  A shallower ring (depth < t_max: whole episodes bounded by the environment's time
+limit, A3C's Mujoco preset cuts every 10^7 steps) refuses a lock-step that would overwrite the first row of a segment
+still open.
 ``observe`` stores one lock-step with one host-to-device copy per column and one ring scatter; ``gather`` copies the
 closed segments' rows (and each segment's last s', the bootstrap state) into the learn buffers with ``cb200_gather``.
 
@@ -27,16 +30,29 @@ def round32(n):
     return max(32, (int(n) + 31) // 32 * 32)
 
 
+def bucket_rows(n):
+    """a learn step's row bucket for n rows: n rounded up to 32 up to 256 rows, above that to a quarter of the power of
+    two below n (256 -> 320 -> 384 -> 448 -> 512 -> 640 -> ...): at most 25 % padding, about 4 log2(rows / 256) + 8
+    sizes"""
+    n = round32(n)
+    if n <= 256:
+        return n
+    step = 1 << ((n - 1).bit_length() - 3)
+    return -(-n // step) * step
+
+
 class LockstepSegments(object):
-    def __init__(self, lib, device, observation_shape, num_envs, t_max, action_dim=None):
-        """action_dim: the action column holds float32 [action_dim] vectors (continuous actions) instead of int64"""
+    def __init__(self, lib, device, observation_shape, num_envs, t_max, action_dim=None, depth=None):
+        """action_dim: the action column holds float32 [action_dim] vectors (continuous actions) instead of int64;
+        depth: rows per stream of the rollout ring and the learn buffers (default t_max)"""
         self.lib = lib
         self.device = dev = torch.device(device)
         obs = tuple(observation_shape)
         self.num_envs = E = int(num_envs)
-        self.t_max = T = int(t_max)
-        if E < 1 or T < 1:
-            raise ValueError("num_envs and num_steps_between_gradient_updates must be >= 1")
+        self.t_max = int(t_max)
+        self.depth = T = self.t_max if depth is None else int(depth)
+        if E < 1 or self.t_max < 1 or T < 1:
+            raise ValueError("num_envs, num_steps_between_gradient_updates and the ring depth must be >= 1")
         obs_dtype = torch.uint8 if len(obs) == 3 else torch.float32
         z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=dev)        # noqa: E731
         self.rollout = {"state": z((T * E,) + obs, obs_dtype), "next_state": z((T * E,) + obs, obs_dtype),
@@ -48,7 +64,7 @@ class LockstepSegments(object):
         pin = dev.type == "cuda"
         self._stage_host = {k: torch.zeros(v.shape, dtype=v.dtype, pin_memory=pin) for k, v in self._stage_dev.items()}
         self._stage_ev = None
-        # learn buffers: at most E * t_max rows close at one step
+        # learn buffers: at most E * depth rows close at one step
         self.max_rows = R = round32(E * T)
         self.learn = {k: z((R,) + tuple(v.shape[1:]), v.dtype) for k, v in self.rollout.items()}
         self.boot_states = z((E,) + obs, obs_dtype)
@@ -75,7 +91,14 @@ class LockstepSegments(object):
     def observe(self, states, actions, rewards, next_states, game_overs):
         """one lock-step of the E streams (agent.py:905-975 observe, core_types.py:716-725 Episode.insert): host
         arrays [E, ...]"""
-        E, T = self.num_envs, self.t_max
+        E, T = self.num_envs, self.depth
+        if T < self.t_max:
+            held = np.minimum(self.episode_length - self.last_gradient_update_step_idx, self.t - self.segment_start)
+            full = np.nonzero(held >= T)[0]
+            if len(full):
+                raise ValueError("stream(s) %s hold %d rows of a segment still open: the rollout ring's depth "
+                                 "(max_episode_steps) is reached before num_steps_between_gradient_updates (%d)"
+                                 % (full.tolist(), T, self.t_max))
         cols = {"state": states, "next_state": next_states, "action": actions, "reward": rewards,
                 "game_over": game_overs}
         if self._stage_ev is not None:
@@ -112,7 +135,7 @@ class LockstepSegments(object):
         """the row-index and segment tables of the segments ``close`` returned, for a bucket of B rows (default: n
         rounded up to 32); returns B.  Only the slots a step of B rows reads are written and copied: the B row slots
         (padding rows read slot 0) and the bootstrap slots."""
-        E, T, t_last = self.num_envs, self.t_max, self.t - 1
+        E, T, t_last = self.num_envs, self.depth, self.t - 1
         n = int(rows.sum())
         B = round32(n) if B is None else int(B)
         if B < n or B > self.max_rows:

@@ -593,6 +593,70 @@ typedef struct cb200_actor_critic_head_desc {
 
 int cb200_actor_critic_head(const cb200_actor_critic_head_desc* ac_desc, void* stream);
 
+/* Actor-critic head for continuous actions (actor_critic_agent.py:111-186, heads/policy_head.py:102-152 with
+ * ContinuousEntropy): ONE Dense(1 + 2 action_dim) on one feature layer, column 0 V, columns 1..D (D = action_dim) the
+ * pre-activation means, D+1..2D the pre-activation stds, over the segment table of cb200_actor_critic_head (segments
+ * must not overlap; rows covered by no segment get zero outputs and dh).
+ *   targets and advantages: cb200_actor_critic_head's A_VALUE / GAE / GAE_VALUE recurrences, the same operations.
+ *   mean = tanh(z) * max_abs_range; std = softplus(z) + FLT_EPSILON with TF 1.x's softplus (x above -t, exp(x) below
+ *   t, log(exp(x) + 1) between, t = log(FLT_EPSILON) + 2); all fp32.
+ *   MultivariateNormalDiag(mean, std) at x = actions[i]: log pi = sum_d [-((x - mean) / std)^2 / 2 - log std -
+ *   log(2 pi) / 2], H = sum_d [(1 + log(2 pi)) / 2 + log std].
+ *   loss = (1/S) sum_s (1/L) sum_i [v_weight l(V_i - target_i) - p_weight log pi_i A_i - beta_entropy H_i] (S the
+ *   non-empty segments), l = squared error or Huber (delta 1); dz = dL/dZ over the 1 + 2D columns (the std columns'
+ *   softplus derivative is sigmoid(z)), dW = h^T dz, db = sum_i dz_i, dh = (dz W^T) relu'(h).
+ * Parallel over rows (a row pass, one thread per segment for the recurrence, a row pass for the loss and dL/dZ);
+ * dW, db and the loss are summed per 64-row chunk, then over the chunks in a fixed order: no atomics on floats, repeat
+ * calls and graph replays give the same bits.  features 256 or 512, action_dim <= 17. */
+typedef struct cb200_actor_critic_gaussian_head_desc {
+    const float* h;             /* [rows, features] post-ReLU features of s                                               */
+    const float* h_boot;        /* [segments, features] features of each segment's last s' (online network)             */
+    const float* w;             /* head kernel [features, 1 + 2 action_dim] and bias [1 + 2 action_dim]                  */
+    const float* b;
+    const float* actions;       /* [rows, action_dim] the actions taken, as fp32                                          */
+    const float* max_abs_range; /* [action_dim]                                                                           */
+    const double* rewards;      /* [rows]                                                                                 */
+    const uint8_t* game_overs;  /* [rows]                                                                                 */
+    const int32_t* seg_offsets; /* [segments]                                                                             */
+    const int32_t* seg_lengths; /* [segments], 0 = unused slot                                                           */
+    int32_t segments;           /* slots in the table, 1 .. 2^20                                                         */
+    int64_t rows;               /* rows of the feature / output buffers, 1 .. 2^24                                       */
+    double discount;
+    double gae_lambda;
+    int32_t mode;               /* CB200_AC_*                                                                             */
+    int32_t huber;              /* VHead loss: 1 tf.losses.huber_loss(delta 1), 0 squared error                           */
+    float beta_entropy;
+    float v_weight;             /* VHead loss weight (0.5)                                                                */
+    float p_weight;             /* PolicyHead loss weight (1.0)                                                           */
+    int32_t features;           /* 256 or 512                                                                             */
+    int32_t action_dim;         /* 1 .. 17                                                                                */
+    float* z;                   /* out [rows, 1 + 2 action_dim]: V | pre-tanh means | pre-softplus stds                   */
+    float* dz;                  /* out, optional [rows, 1 + 2 action_dim]: dL/dZ                                          */
+    float* loss;                /* out scalar, optional                                                                   */
+    float* means;               /* out, optional [rows, action_dim]                                                       */
+    float* stds;                /* out, optional [rows, action_dim]                                                       */
+    float* targets;             /* out, optional [rows]: V targets (fp32)                                                 */
+    float* advantages;          /* out, optional [rows] (fp32)                                                            */
+    float* bootstrap;           /* out, optional [segments]: V(s'_last), 0 after a terminal state                        */
+    float* dh;                  /* out, optional: [rows, features] dL/d(pre-activation of the feature layer)             */
+    void* dh_planes;            /* out, optional: the same as tiled bf16 hi / mid / lo planes                             */
+    int64_t dh_plane_stride;
+    float* dw;                  /* out [features, 1 + 2 action_dim]                                                       */
+    float* db;                  /* out [1 + 2 action_dim]                                                                 */
+    float* workspace;           /* rows * (2 action_dim + 5) + segments + ceil(rows / 64) * (features + 1) *
+                                   (2 action_dim + 1) + ceil(rows / 64) floats                                            */
+} cb200_actor_critic_gaussian_head_desc;
+
+int cb200_actor_critic_gaussian_head(const cb200_actor_critic_gaussian_head_desc* acg_desc, void* stream);
+
+/* Acting from the continuous actor-critic head's outputs z [envs, 1 + 2 action_dim] (ContinuousEntropy, i.e.
+ * exploration_policies/additive_noise.py:74-103 with the network's std): mean and std with the head's code (fp32);
+ * with normals [envs, action_dim] (np.random.standard_normal) the action is numpy's normal(mean, std) =
+ * (double) mean + (double) std * normal in fp64; normals NULL (evaluation): the mean.  actions [envs, action_dim] fp64
+ * out; means and stds [envs, action_dim] fp32 out, optional. */
+int cb200_gaussian_policy_act(const float* z, int64_t envs, int32_t action_dim, const float* max_abs_range,
+                              const double* normals, double* actions, float* means, float* stds, void* stream);
+
 /* Categorical acting (exploration_policies/categorical.py:36-47): z [envs, 1 + n_actions] as the actor-critic head
  * lays it out (V | logits); p = softmax(logits) with the head's code.  uniforms [envs] (np.random.random_sample):
  * np.random.choice's draw, cdf = cumsum(double(p)) in index order, cdf /= cdf[-1], action = the number of entries
