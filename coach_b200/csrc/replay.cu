@@ -1314,8 +1314,12 @@ static int launch_gather_s2d(const SampleParams& sp, const int64_t* idx_in, int6
     static size_t configured = 0;
     if (smem > configured) {
         if (cudaFuncSetAttribute(sample_gather_s2d_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
-            cudaSuccess)
+            cudaSuccess) {
+            // more than a CTA can hold: the caller refuses the geometry; clear the error so that the next launch's
+            // check does not report it
+            cudaGetLastError();
             return -1;
+        }
         configured = smem;
     }
     CB200_LAUNCH(sample_gather_s2d_kernel, (unsigned)(groups * parts), kS2dThreads, smem, st, sp, gp, tmF);
@@ -1327,6 +1331,8 @@ static int check_s2d_args(const cb200_column* img, int n_img, int64_t n, int h, 
     if (!img || n_img < 1 || n_img > 2 || n <= 0 || n % 8 != 0) return -1;
     if (s <= 0 || h % s || w % s || (s * c) % 8 != 0 || ((int64_t)s * w * c) % 16 != 0 || ((int64_t)h * w * c) % 16 != 0)
         return -1;
+    // the conversion gives each s2d pixel 8 * s threads: beyond s = 32 a CTA has no thread for a pixel
+    if (8 * s > kS2dThreads) return -1;
     if (n_small < 0 || n_small > CB200_MAX_COLUMNS || (n_small > 0 && !small_cols)) return -1;
     // frame-deduplicated ring: 4 x 4 space-to-depth blocks of 4-frame stacks; frames and their row bands 16-byte aligned
     if (frames && (s != 4 || c != 4 || ((int64_t)h * w) % 16 != 0 || ((int64_t)s * w) % 16 != 0 ||
@@ -1352,7 +1358,7 @@ int cb200_per_sample_gather_s2d(const double* sum_tree, const double* min_tree, 
                     "bad arguments (size must be a power of 2, n > 0, non-null trees / uniforms)");
     CB200_CHECK_ARG(idx_out != nullptr, "idx_out is required");
     CB200_CHECK_ARG(check_s2d_args(image_columns, n_image, n, h, w, c, s, small_columns, n_small, frames) == 0,
-                    "bad image geometry / column table (n % 8 == 0, 1-2 uint8 image columns, 16-byte aligned rows)");
+                    "bad image geometry / column table (n % 8 == 0, s <= 32, 1-2 uint8 image columns, 16-byte aligned rows)");
     const int rc = launch_gather_s2d(sp, nullptr, n, image_columns, n_image, h, w, c, s, small_columns, n_small,
                                      frames, frame_slots, as_stream(stream));
     CB200_CHECK_ARG(rc == 0, "could not configure the fused sample + gather + space-to-depth kernel");
@@ -1365,7 +1371,7 @@ int cb200_gather_s2d(const int64_t* idx, int64_t n, const cb200_column* image_co
                      int64_t frame_slots, void* stream) {
     CB200_CHECK_ARG(idx != nullptr, "idx is required");
     CB200_CHECK_ARG(check_s2d_args(image_columns, n_image, n, h, w, c, s, small_columns, n_small, frames) == 0,
-                    "bad image geometry / column table (n % 8 == 0, 1-2 uint8 image columns, 16-byte aligned rows)");
+                    "bad image geometry / column table (n % 8 == 0, s <= 32, 1-2 uint8 image columns, 16-byte aligned rows)");
     SampleParams sp;
     memset(&sp, 0, sizeof(sp));
     const int rc = launch_gather_s2d(sp, idx, n, image_columns, n_image, h, w, c, s, small_columns, n_small, frames,

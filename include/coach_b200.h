@@ -146,7 +146,9 @@ int cb200_per_sample_gather(const double* sum_tree, const double* min_tree, int6
  *   image_columns[k]: src = ring column (uint8 [capacity, h*w*c]), dst = plane (bf16 [(h/s)*(w/s)*n, s*s*c],
  *                     core-tiled), row_bytes = h*w*c; 1 or 2 columns (state, next_state)
  *   small_columns   : the remaining columns, copied row by row into their staged [n, row_bytes] buffers
- * n must be a multiple of 8 (whole 8-row groups of the plane matrix).  idx_out / w_out / w32_out as cb200_per_sample.
+ * n must be a multiple of 8 (whole 8-row groups of the plane matrix).  s is at most 32 (8*s threads convert one s2d
+ * pixel, 256 per CTA), and an s2d row of s*w*c bytes above about 14.5 KB needs more than the 227 KiB of shared memory
+ * a CTA can hold: both are refused (CB200_ERR_INVALID_ARGUMENT).  idx_out / w_out / w32_out as cb200_per_sample.
  * Frame-deduplicated ring (`frames` != NULL, s == c == 4): the ring stores every h x w frame ONCE in `frames`
  * (uint8 [frame slots, h*w]) -- the reference shares them between s, s' and neighbouring transitions through LazyStack
  * (filters/observation/observation_stacking_filter.py:27-41, agents/agent.py:905-973); image_columns[k].src is then the

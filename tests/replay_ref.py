@@ -1,7 +1,8 @@
 """Host references of the replay kernels of include/coach_b200.h (coach_b200/csrc/replay.cu, and cb200_gather_at in
-heads.cu): the launch-plan mirrors that tell which regime a call runs in, the exact references of the row copies, and
-the segment-tree references, which run oracle/segment_tree.c through oracle.memory.  numpy only, importable without
-CUDA.
+heads.cu): the launch-plan mirrors that tell which regime a call runs in (the row gathers and the fused sample +
+gather + space-to-depth kernel), the exact references of the row copies, and the segment-tree references, which run
+oracle/segment_tree.c through oracle.memory.  The space-to-depth planes themselves are tests/learn_ref.u8_s2d_plane of
+the gathered frames.  numpy only, importable without CUDA.
 
 Bounds: tree nodes, leaf indices, raw priorities and every copied byte are bit for bit; importance weights within 4 ulp
 of the oracle (both ends call pow); p_alpha from the device's pow within 2 ulp of Python's `**`, from the host's libm
@@ -205,6 +206,116 @@ def descent_rounds(size):
     while levels > 0:
         out.append(min(levels, ROUND_LEVELS))
         levels -= out[-1]
+    return out
+
+
+# replay.cu:689-690, :1284-1313: the fused sample + gather + space-to-depth kernel
+S2D_THREADS = 256             # kS2dThreads
+S2D_STAGES = 2                # kS2dStages
+S2D_CHUNK_BUDGET = 2816       # bytes of s2d rows per sample and chunk
+S2D_SCRATCH = 256 + 8 * 256 * 8     # phase A: the per-warp descent scratch (kScratchDoubles doubles per warp)
+SMEM_DEFAULT = 48 * 1024      # dynamic shared memory a launch gets without the opt-in attribute
+SMEM_OPTIN = 227 * 1024       # the opt-in limit of one H100 CTA
+TMA_BOX_WORDS = 256           # largest TMA box dimension
+
+
+def s2d_plan(n, n_img, h, w, c, s, sm_count, frames=False, frame_slots=0, frame_tma_knob=0):
+    """replay.cu:1282-1311 launch_gather_s2d (and :1229-1260 frame_store_map), :729-736 / :755 / :805-828 of the kernel.
+
+    CTA = (8-sample group, image column, band of s2d rows): `parts` bands of `per_band` rows, as many CTAs as one wave
+    of four per SM holds; each band is streamed in chunks of `rows_per_chunk` s2d rows (about 2816 bytes per sample)
+    through two shared-memory stages of 8 * `chunk_stride` bytes.  The frame store fetches a stack of four
+    consecutive frame slots with one 2-D TMA box when the knob is on, the per-sample stride is a multiple of 128 bytes
+    and the box is at most 256 words wide.  Conversion: 8 S threads per s2d pixel, `slots` pixels per pass, pixel
+    index advanced by (dyl rows, dX columns) -- 'multi-pass' when a chunk has more pixels than slots ('-dyl' when a
+    step crosses whole rows).  `bands` holds (chunks, last chunk partial) per band; `regimes` names
+    what the call exercises; `refusal` names why the library refuses the geometry (None: it launches)."""
+    hs, ws = h // s, w // s
+    row = s * w * c                                   # s2d_row_bytes: one s2d row of one sample
+    groups = n // 8 * n_img
+    parts = min(max(4 * sm_count // groups, 1), hs)
+    per_band = _cdiv(hs, parts)
+    rc = min(max(S2D_CHUNK_BUDGET // row, 1), per_band)
+    stride = rc * row
+    band_bytes = rc * s * w                           # frame store: bytes of one frame's band of a chunk
+    tma_eligible = bool(frames) and frame_slots >= 4 and stride % 128 == 0
+    frame_tma = tma_eligible and bool(frame_tma_knob) and band_bytes // 4 <= TMA_BOX_WORDS
+    if not frame_tma and (stride // 16) % 2 == 0:
+        stride += 16
+    smem = max(256 + S2D_STAGES * 8 * stride, S2D_SCRATCH)
+    slots = S2D_THREADS // (8 * s)
+    dyl, dX = divmod(slots, ws) if slots else (0, 0)
+    bands = []
+    for p in range(parts):
+        rows = max(min(hs, (p + 1) * per_band) - p * per_band, 0)
+        bands.append((_cdiv(rows, rc), rows % rc != 0))
+    refusal = "s>32" if slots == 0 else ("smem" if smem > SMEM_OPTIN else None)
+    reg = set()
+    chunks = [k for k, _ in bands if k]
+    if max(chunks) == 1:
+        reg.add("one-chunk")
+    if max(chunks) > S2D_STAGES:
+        reg.add("refill")
+    if any(part for _, part in bands):
+        reg.add("partial")
+    if min(k for k, _ in bands) == 0:
+        reg.add("empty-band")
+    if parts == 1:
+        reg.add("one-band")
+    if parts == hs and hs > 1:
+        reg.add("bands=Hs")
+    if row > S2D_CHUNK_BUDGET:
+        reg.add("rc=1")
+    if smem > SMEM_DEFAULT:
+        reg.add("smem>48K")
+    if frames:
+        reg.add("tma" if frame_tma else ("tma-ineligible" if frame_tma_knob else "bulk"))
+    else:
+        run = s * c
+        reg.add("run=16" if run == 16 else ("run=8" if run == 8 else "run=8k"))
+        reg.add("S=%d" % s)
+        if S2D_THREADS % (8 * s):
+            reg.add("idle-threads")
+        if slots > ws:
+            reg.add("slots>Ws")
+        if ws == 1:
+            reg.add("Ws=1")
+        if rc * ws > slots > 0:
+            reg.add("multi-pass" if dyl == 0 else "multi-pass-dyl")
+    return dict(parts=parts, per_band=per_band, rows_per_chunk=rc, chunk_stride=stride, smem=smem,
+                frame_tma=frame_tma, slots=slots, dyl=dyl, dX=dX, bands=bands, grid=groups * parts, regimes=reg,
+                refusal=refusal)
+
+
+def s2d_chunk_full(plan):
+    """per chunk of every band, in (band, chunk) order: whether it holds rows_per_chunk rows (False: the partial last
+    chunk of a band)"""
+    out = []
+    for k, partial in plan["bands"]:
+        out += [True] * (k - 1) + [not partial] if k else []
+    return np.array(out, bool)
+
+
+def s2d_one_box(fidx_rows, rc_full):
+    """replay.cu:773-774: with frame_tma on, sample i fetches chunk j with one 2-D TMA box when its stack sits in four
+    consecutive frame slots and the chunk is full; otherwise with four per-frame bulk copies.  fidx_rows: the [n, 4]
+    frame slots of the sampled stacks; rc_full: s2d_chunk_full.  Returns bool [n, chunks]."""
+    f = np.asarray(fidx_rows, np.int64)
+    consecutive = (f[:, 1] == f[:, 0] + 1) & (f[:, 2] == f[:, 0] + 2) & (f[:, 3] == f[:, 0] + 3)
+    return consecutive[:, None] & np.asarray(rc_full, bool)[None, :]
+
+
+def s2d_box_regimes(one_box, rc_full):
+    """the copy paths a frame-store call takes: 'one-box', 'four-copies' (a stack not in consecutive slots) and
+    'partial-fallback' (a consecutive stack copied frame by frame because the chunk is partial)"""
+    out = set()
+    if one_box.any():
+        out.add("one-box")
+    consecutive = one_box.any(axis=1)
+    if (~consecutive).any():
+        out.add("four-copies")
+    if consecutive.any() and (~np.asarray(rc_full, bool)).any():
+        out.add("partial-fallback")
     return out
 
 

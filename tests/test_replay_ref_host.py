@@ -1,9 +1,11 @@
 """Pins tests/replay_ref.py (no GPU): the launch-plan mirrors against plans worked out by hand from replay.cu, the
 protocol model of the bulk-copy pipeline (which plans hung before the one-stage fix, and that none does now), the
-regimes the GPU test's cases reach, and the tree references against the sequential C oracle."""
+regimes the GPU tests' cases reach, the tree references against the sequential C oracle, and the space-to-depth mirror
+and plane reference of the fused sample + gather + space-to-depth kernel."""
 import numpy as np
 import pytest
 
+import learn_ref as lr
 import replay_cases as rc
 import replay_ref as rr
 
@@ -185,3 +187,141 @@ def test_oracle_store_wraps_at_the_cursor():
 def test_host_priorities_reference():
     pa, pr = rr.host_priorities([0.0, 1.5, -0.5, np.nan], 1e-6, 0.6)
     assert pr[0] == 1e-6 and pa[1] == (1.5 + 1e-6) ** 0.6 and np.isnan(pa[2:]).all() and np.isnan(pr[2:]).all()
+
+
+# ---- the fused sample + gather + space-to-depth kernel -------------------------------------------------------------------
+# (n, n_img, sm) -> (parts, per_band, rows_per_chunk, chunk_stride, smem, bands) for Atari frames (84x84x4, s = 4: 21 s2d
+# rows of 1344 bytes, 2816 // 1344 = 2 rows per chunk); parts = min(4 sm // (n / 8 * n_img), 21); a stride of an even
+# number of 16-byte units gets 16 bytes of padding; smem = 256 + 2 stages * 8 samples * stride
+ATARI_S2D = {
+    (8, 1, 132): (21, 1, 1, 1360, 22016, [(1, False)] * 21),          # 1344 = 84 x 16 -> 1360; the 16640-byte scratch
+    (128, 2, 132): (16, 2, 2, 2704, 43520, [(1, False)] * 10 + [(1, True)] + [(0, False)] * 5),  # 528 // 32 = 16
+    (512, 1, 132): (8, 3, 2, 2704, 43520, [(2, True)] * 7 + [(0, False)]),                       # 528 // 64 = 8
+    (512, 2, 132): (4, 6, 2, 2704, 43520, [(3, False)] * 3 + [(2, True)]),                       # a stage refill
+    (4096, 1, 132): (1, 21, 2, 2704, 43520, [(11, True)]),
+    (128, 2, 114): (14, 2, 2, 2704, 43520, [(1, False)] * 10 + [(1, True)] + [(0, False)] * 3),  # 456 // 32 = 14
+    (512, 2, 114): (3, 7, 2, 2704, 43520, [(4, True)] * 3),                                      # 456 // 128 = 3
+}
+
+
+@pytest.mark.parametrize("key", sorted(ATARI_S2D))
+def test_s2d_atari_plans_by_hand(key):
+    n, n_img, sm = key
+    p = rr.s2d_plan(n, n_img, 84, 84, 4, 4, sm)
+    parts, per_band, rows, stride, smem, bands = ATARI_S2D[key]
+    assert (p["parts"], p["per_band"], p["rows_per_chunk"], p["chunk_stride"], p["smem"]) == (
+        parts, per_band, rows, stride, smem)
+    assert p["bands"] == bands and p["grid"] == n // 8 * n_img * parts and p["refusal"] is None
+    assert (p["slots"], p["dyl"], p["dX"], p["frame_tma"]) == (8, 0, 8, False)        # 32 threads per pixel, 21 columns
+    assert sum(k * rows - part for k, part in bands) == 21                              # every s2d row exactly once
+    reg = p["regimes"]
+    assert ("empty-band" in reg) == any(k == 0 for k, _ in bands)
+    assert ("partial" in reg) == any(part for _, part in bands)
+    assert ("refill" in reg) == (max(k for k, _ in bands) > rr.S2D_STAGES)
+
+
+def test_s2d_frame_store_plans_by_hand():
+    # 84x84 at B = 128, two columns: 2688 = 21 x 128 bytes per sample, a 672-byte (168-word) band: TMA boxes, no padding
+    p = rr.s2d_plan(128, 2, 84, 84, 4, 4, SM, True, 64, 1)
+    assert p["frame_tma"] and p["chunk_stride"] == 2688 and p["smem"] == 256 + 16 * 2688
+    assert list(rr.s2d_chunk_full(p)) == [True] * 10 + [False]
+    assert not rr.s2d_plan(128, 2, 84, 84, 4, 4, SM, True, 64, 0)["frame_tma"]           # knob off
+    assert not rr.s2d_plan(128, 2, 84, 84, 4, 4, SM, True, 3, 1)["frame_tma"]            # fewer than four slots
+    assert rr.s2d_plan(32, 1, 16, 16, 4, 4, SM, True, 4, 1)["frame_tma"]                 # exactly four slots
+    # one s2d row per chunk: 1344 bytes per sample is not a multiple of 128 -> bulk copies, 16 bytes of padding
+    p = rr.s2d_plan(8, 1, 84, 84, 4, 4, SM, True, 64, 1)
+    assert not p["frame_tma"] and p["chunk_stride"] == 1360 and "tma-ineligible" in p["regimes"]
+    # 8x272 frames: 4352 = 34 x 128 bytes per sample, but a 1088-byte band is 272 words, wider than a TMA box
+    p = rr.s2d_plan(8, 1, 8, 272, 4, 4, SM, True, 64, 1)
+    assert not p["frame_tma"] and p["chunk_stride"] == 4368 and p["rows_per_chunk"] == 1
+
+
+def test_s2d_conversion_and_refusals_by_hand():
+    p = rr.s2d_plan(1024, 1, 48, 12, 8, 3, SM)          # 24 threads per pixel: 10 slots, 16 idle threads, 4 columns
+    assert (p["slots"], p["dyl"], p["dX"], p["rows_per_chunk"]) == (10, 2, 2, 4)
+    assert {"idle-threads", "slots>Ws", "multi-pass-dyl", "run=8k"} <= p["regimes"]
+    p = rr.s2d_plan(8, 1, 64, 32, 1, 32, SM)            # 256 threads per pixel: one slot, w / s == 1
+    assert (p["slots"], p["dyl"], p["dX"]) == (1, 1, 0) and p["refusal"] is None and "Ws=1" in p["regimes"]
+    p = rr.s2d_plan(*rc.S2D_S64, SM)                    # 512 threads per pixel: no slot, the planes would stay unwritten
+    assert p["slots"] == 0 and p["refusal"] == "s>32"
+    p = rr.s2d_plan(16, 1, 8, 256, 4, 4, SM)            # 4096-byte s2d rows: one per chunk, 4112-byte stride
+    assert (p["rows_per_chunk"], p["chunk_stride"], p["smem"]) == (1, 4112, 66048)
+    assert rr.s2d_plan(8, 1, 4, 896, 4, 4, SM)["smem"] == 256 + 16 * 14352 <= rr.SMEM_OPTIN
+    p = rr.s2d_plan(*rc.S2D_OVER_SMEM, SM)
+    assert p["smem"] == 256 + 16 * 16400 > rr.SMEM_OPTIN and p["refusal"] == "smem"
+
+
+def test_s2d_one_box_by_hand():
+    rows = [(0, 1, 2, 3), (5, 5, 5, 5), (5, 5, 6, 7), (62, 63, 0, 1), (60, 61, 62, 63), (7, 8, 9, 9)]
+    full = [True, True, False]
+    got = rr.s2d_one_box(rows, full)
+    want = np.array([[1, 1, 0], [0, 0, 0], [0, 0, 0], [0, 0, 0], [1, 1, 0], [0, 0, 0]], bool)
+    np.testing.assert_array_equal(got, want)
+    assert rr.s2d_box_regimes(got, full) == {"one-box", "four-copies", "partial-fallback"}
+    assert rr.s2d_box_regimes(rr.s2d_one_box(rows[:1], [True]), [True]) == {"one-box"}
+    assert rr.s2d_box_regimes(rr.s2d_one_box(rows[1:4], full), full) == {"four-copies"}
+
+
+def test_frame_tables_hold_every_stack_kind():
+    for slots in (64, 4):
+        fidx = rc.frame_table(np.random.RandomState(0), rc.S2D_FRAME_CAPACITY, slots)
+        assert fidx.shape == (rc.S2D_FRAME_CAPACITY, 4) and fidx.min() >= 0 and fidx.max() < slots
+        f = rc.frame_idx(np.random.RandomState(1), 8, fidx)
+        s = fidx[f[:4]].astype(np.int64)
+        assert (np.diff(s[0]) == 1).all() and (np.diff(s[1]) == 0).all()
+        assert list(np.diff(s[2])) == [0, 1, 1] and (np.diff(s[3]) < 0).any()
+
+
+def _s2d_table_regimes(sm):
+    """the regimes the GPU test's case table reaches on `sm` multiprocessors, named as the test names them"""
+    ran = set()
+    for n, n_img, h, w, c, s, small in rc.S2D_RING:
+        p = rr.s2d_plan(n, n_img, h, w, c, s, sm)
+        assert p["refusal"] is None
+        ran |= {("ring", r) for r in p["regimes"]}
+        spec = rc.SMALL_MIX if small == "mix" else ()
+        ran |= {("copy", rr.copy_path(off, off, rb)) for rb, off in spec} | {("small", len(spec))}
+    for n, n_img, h, w, slots, _ in rc.S2D_FRAMES:
+        rng = np.random.RandomState(n + h + slots)
+        fidx = rc.frame_table(rng, rc.S2D_FRAME_CAPACITY, slots)
+        rows = fidx[rc.frame_idx(rng, n, fidx)]
+        for knob in (0, 1):
+            p = rr.s2d_plan(n, n_img, h, w, 4, 4, sm, True, slots, knob)
+            ran |= {("frames", r) for r in p["regimes"]}
+            if p["frame_tma"]:
+                full = rr.s2d_chunk_full(p)
+                ran |= {("box", r) for r in rr.s2d_box_regimes(rr.s2d_one_box(rows, full), full)}
+    for size, n, n_img, h, w, c, s, frames, outs in rc.S2D_PER:
+        p = rr.s2d_plan(n, n_img, h, w, c, s, sm, frames, 64 if frames else 0)
+        ran |= {("frames" if frames else "ring", r) for r in p["regimes"]}
+        ran |= {("per", o) for o in outs or ("no-weights",)} | {("per", "size=%d" % size)}
+        ran |= {("per", "frames")} if frames else set()
+    return ran
+
+
+@pytest.mark.parametrize("sm", [132, 114])
+def test_s2d_case_table_reaches_every_regime(sm):
+    """on an H100 SXM (132 SMs) and PCIe (114 SMs) the case table reaches every regime the GPU test requires; the
+    regimes the frame-store cases reach with the TMA boxes on come from the sampled stacks"""
+    missing = rc.S2D_REQUIRED - _s2d_table_regimes(sm)
+    assert not missing, sorted(missing)
+
+
+@pytest.mark.parametrize("B,h,w,c,s", [(8, 6, 10, 8, 1), (8, 4, 6, 16, 1), (8, 9, 12, 8, 3), (8, 10, 20, 8, 5),
+                                       (16, 12, 12, 4, 6), (8, 16, 16, 1, 8), (8, 64, 32, 1, 32), (8, 8, 8, 2, 4)])
+def test_u8_s2d_plane_against_a_plain_loop(B, h, w, c, s):
+    """learn_ref.u8_s2d_plane against the definition, element by element: pixel (y, x, ch) of sample b goes to plane
+    row (y / s * (w / s) + x / s) * B + b, column ((y % s) s + x % s) c + ch, of the 8x8 core-tiled layout, as the bf16
+    bits of its value (the upper half of the fp32)"""
+    x = np.random.RandomState(B + h + s).randint(0, 256, (B, h, w, c)).astype(np.uint8)
+    ws, cs = w // s, s * s * c
+    want = np.zeros(h * w * c * B, np.uint16)
+    for b in range(B):
+        for y in range(h):
+            for xx in range(w):
+                for ch in range(c):
+                    r = (y // s * ws + xx // s) * B + b
+                    col = ((y % s) * s + xx % s) * c + ch
+                    e = ((r // 8) * (cs // 8) + col // 8) * 64 + (r % 8) * 8 + col % 8
+                    want[e] = np.float32(x[b, y, xx, ch]).view(np.uint32) >> 16
+    np.testing.assert_array_equal(lr.u8_s2d_plane(x, s), want)
