@@ -234,7 +234,9 @@ class ClippedPPOAgent(object):
         world = parallel.world()[1]
         graphable = self.use_cuda_graph and self.device.type == "cuda" and world == 1
         if graphable:
-            # warm-up launch outside capture (lazy module loading), then capture once
+            # warm-up launch outside capture (lazy module loading), then capture once.  The warm-up gathers at the
+            # cursor, which a previous phase left at its rollout's end: start it at row 0, inside this permutation.
+            self.cursor.zero_()
             side = torch.cuda.Stream()
             side.wait_stream(torch.cuda.current_stream())
             with torch.cuda.stream(side):

@@ -23,6 +23,23 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
     return out;
 }
 
+// Per-element Gaussian terms of the two PPO heads (clipped and KL-penalty): sigma = exp(logstd) + eps, one dimension's
+// KL(old || new) of diagonal Gaussians, the log-likelihood from its squared-z sum, the entropy and d sigma / d logstd
+// over sigma.
+__device__ __forceinline__ float ppo_sigma(float logstd) { return expf(logstd) + kTfEps; }
+__device__ __forceinline__ float ppo_kl_term(float m, float old_m, float sig, float old_sig) {
+    const float dm = (m - old_m) / sig;
+    const float rs = old_sig / sig;
+    return 0.5f * (rs * rs + dm * dm - 1.0f) - logf(rs);
+}
+__device__ __forceinline__ float ppo_logp(float q, float sum_log_sig, int A) {
+    return -0.5f * q - sum_log_sig - 0.5f * A * kLog2Pi;
+}
+__device__ __forceinline__ float ppo_entropy(int A, float sum_log_sig) {
+    return 0.5f * A * (1.0f + kLog2Pi) + sum_log_sig;
+}
+__device__ __forceinline__ float ppo_dsig(float sig) { return (sig - kTfEps) / sig; }
+
 // =====================================================================================================================
 // PPOHead, continuous actions (heads/ppo_head.py:52-144): diagonal Gaussian with state-independent log-std.
 //   sigma_j   = exp(logstd_j) + eps
@@ -40,8 +57,8 @@ __global__ void __launch_bounds__(256) ppo_continuous_head_kernel(
     __shared__ float red[256];
     __shared__ float sig[kMaxActionDim], osig[kMaxActionDim], dls_part[kMaxActionDim];
     if (threadIdx.x < A) {
-        sig[threadIdx.x] = expf(logstd[threadIdx.x]) + kTfEps;
-        osig[threadIdx.x] = expf(old_logstd[threadIdx.x]) + kTfEps;
+        sig[threadIdx.x] = ppo_sigma(logstd[threadIdx.x]);
+        osig[threadIdx.x] = ppo_sigma(old_logstd[threadIdx.x]);
         dls_part[threadIdx.x] = 0.f;
     }
     __syncthreads();
@@ -64,13 +81,10 @@ __global__ void __launch_bounds__(256) ppo_continuous_head_kernel(
             const float zo = (a - old_mu[i * A + j]) / osig[j];
             q += z * z;
             qo += zo * zo;
-            // KL(old || new) of diagonal Gaussians
-            const float dm = (mu[i * A + j] - old_mu[i * A + j]) / sig[j];
-            const float rs = osig[j] / sig[j];
-            kl += 0.5f * (rs * rs + dm * dm - 1.0f) - logf(rs);
+            kl += ppo_kl_term(mu[i * A + j], old_mu[i * A + j], sig[j], osig[j]);
         }
-        const float logp = -0.5f * q - sum_log_sig - 0.5f * A * kLog2Pi;
-        const float logp_old = -0.5f * qo - sum_log_osig - 0.5f * A * kLog2Pi;
+        const float logp = ppo_logp(q, sum_log_sig, A);
+        const float logp_old = ppo_logp(qo, sum_log_osig, A);
         const float ratio = expf(logp - logp_old);
         const float cl = fminf(fmaxf(ratio, lo), hi);
         const float adv = advantages[i];
@@ -88,7 +102,7 @@ __global__ void __launch_bounds__(256) ppo_continuous_head_kernel(
             const float z = (actions[i * A + j] - mu[i * A + j]) / sig[j];
             d_mu[i * A + j] = dlogp * z / sig[j];
             // d logp / d logstd_j = (z^2 - 1) * exp(logstd_j) / sigma_j
-            dls_local[j] += dlogp * (z * z - 1.0f) * ((sig[j] - kTfEps) / sig[j]);
+            dls_local[j] += dlogp * (z * z - 1.0f) * ppo_dsig(sig[j]);
         }
     }
     const float loss_sum = block_sum(loss_acc, red);
@@ -101,10 +115,10 @@ __global__ void __launch_bounds__(256) ppo_continuous_head_kernel(
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        const float entropy = 0.5f * A * (1.0f + kLog2Pi) + sum_log_sig;     // state independent
+        const float entropy = ppo_entropy(A, sum_log_sig);     // state independent
         for (int j = 0; j < A; ++j) {
             // entropy regulariser -beta * H:  dH/dlogstd_j = exp(logstd_j) / sigma_j
-            d_logstd[j] = dls_part[j] - beta_entropy * ((sig[j] - kTfEps) / sig[j]);
+            d_logstd[j] = dls_part[j] - beta_entropy * ppo_dsig(sig[j]);
         }
         if (scalars) {
             scalars[0] = -loss_sum * inv_b - beta_entropy * entropy;
@@ -731,6 +745,122 @@ __global__ void __launch_bounds__(128) qr_q_values_kernel(const float* __restric
     if (lane == 0) q[r] = v;
 }
 
+// =====================================================================================================================
+// PPOHead with the KL penalty instead of clipping (heads/ppo_head.py:64-97 with clip_likelihood_ratio_using_epsilon
+// None): per minibatch of B rows
+//   KLbar = mean_i KL_i(old || new),   ratio_i = exp(logp_i - logp_old_i)
+//   L     = -mean_i ratio_i * A_i  +  use_kl * (k * KLbar + c * max(0, KLbar - cutoff)^2)  -  beta * H
+// so every row's gradient depends on KLbar through f = k + 2 c max(0, KLbar - cutoff):
+//   dL/dmu_ij     = (-A_i ratio_i z_ij + f dm_ij) / (B sigma_j),              z = (a - mu) / sigma, dm = (mu - mu_old) / sigma
+//   dL/dlogstd_j  = [sum_i (-A_i ratio_i (z_ij^2 - 1) + f (1 - rs_j^2 - dm_ij^2)) / B - beta] (sigma_j - eps) / sigma_j,
+//                   rs = sigma_old / sigma
+// One CTA.  A warp owns a row at a time, lane j its dimension j (A <= 32), so the per-row sums are xor-shuffle trees
+// whose result every lane holds bit for bit.  Pass 1 forms KLbar, pass 2 the gradients and the logged scalars.  Each
+// warp accumulates its rows in order and the warps' partials are summed in warp order: no atomics, so repeat calls and
+// graph replays give identical bits.  k is read from device memory so a captured graph follows coefficient updates.
+// =====================================================================================================================
+constexpr int kPpoKlThreads = 1024;
+constexpr int kPpoKlWarps = kPpoKlThreads / 32;
+
+__global__ void __launch_bounds__(kPpoKlThreads) ppo_kl_head_kernel(
+    const float* __restrict__ mu, const float* __restrict__ logstd, const float* __restrict__ actions,
+    const float* __restrict__ old_mu, const float* __restrict__ old_logstd, const float* __restrict__ advantages,
+    int64_t B, int A, const float* __restrict__ kl_coef, float kl_cutoff, float high_kl_penalty, int use_kl,
+    float beta_entropy, float* __restrict__ d_mu, float* __restrict__ d_logstd,
+    float* __restrict__ scalars /* [loss, KLbar, entropy, mean ratio, surrogate] */) {
+    __shared__ float dls_part[kPpoKlWarps][kMaxActionDim];
+    __shared__ float row_part[3][kPpoKlWarps];          // per warp: KL, ratio, ratio * advantage
+    __shared__ float kl_mean_s;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool on = lane < A;
+    const float sig = on ? ppo_sigma(logstd[lane]) : 1.f;
+    const float osig = on ? ppo_sigma(old_logstd[lane]) : 1.f;
+    const float sum_log_sig = warp_sum(on ? logf(sig) : 0.f);
+    const float sum_log_osig = warp_sum(on ? logf(osig) : 0.f);
+    const float inv_b = 1.0f / (float)B;
+
+    float kl_acc = 0.f;
+    for (int64_t i = warp; i < B; i += kPpoKlWarps) {
+        const float t = on ? ppo_kl_term(mu[i * A + lane], old_mu[i * A + lane], sig, osig) : 0.f;
+        kl_acc += warp_sum(t);
+    }
+    if (lane == 0) row_part[0][warp] = kl_acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int w = 0; w < kPpoKlWarps; ++w) s += row_part[0][w];
+        kl_mean_s = s * inv_b;
+    }
+    __syncthreads();
+    const float kl_mean = kl_mean_s;
+    const float excess = fmaxf(0.f, kl_mean - kl_cutoff);
+    const float coef = use_kl ? *kl_coef : 0.f;
+    const float f_over_b = use_kl ? (coef + 2.0f * high_kl_penalty * excess) * inv_b : 0.f;
+
+    float dls = 0.f, ratio_acc = 0.f, surr_acc = 0.f;
+    for (int64_t i = warp; i < B; i += kPpoKlWarps) {
+        float z = 0.f, zo = 0.f, dm = 0.f;
+        if (on) {
+            const float a = actions[i * A + lane], m = mu[i * A + lane], om = old_mu[i * A + lane];
+            z = (a - m) / sig;
+            zo = (a - om) / osig;
+            dm = (m - om) / sig;
+        }
+        const float q = warp_sum(z * z), qo = warp_sum(zo * zo);
+        const float ratio = expf(ppo_logp(q, sum_log_sig, A) - ppo_logp(qo, sum_log_osig, A));
+        const float adv = advantages[i];
+        ratio_acc += ratio;
+        surr_acc += ratio * adv;
+        const float dlogp = -inv_b * adv * ratio;          // dL/dlogp_i
+        if (on) {
+            const float rs = osig / sig;
+            d_mu[i * A + lane] = (dlogp * z + f_over_b * dm) / sig;
+            dls += dlogp * (z * z - 1.0f) + f_over_b * (1.0f - rs * rs - dm * dm);
+        }
+    }
+    if (on) dls_part[warp][lane] = dls;
+    if (lane == 0) {
+        row_part[1][warp] = ratio_acc;
+        row_part[2][warp] = surr_acc;
+    }
+    __syncthreads();
+    if (threadIdx.x < A) {
+        float s = 0.f;
+        for (int w = 0; w < kPpoKlWarps; ++w) s += dls_part[w][threadIdx.x];
+        const float ds = ppo_dsig(sig);
+        d_logstd[threadIdx.x] = s * ds - beta_entropy * ds;
+    }
+    if (threadIdx.x == 0 && scalars) {
+        float r = 0.f, sa = 0.f;
+        for (int w = 0; w < kPpoKlWarps; ++w) {
+            r += row_part[1][w];
+            sa += row_part[2][w];
+        }
+        const float entropy = ppo_entropy(A, sum_log_sig);
+        const float surrogate = -sa * inv_b;
+        const float penalty = use_kl ? coef * kl_mean + high_kl_penalty * excess * excess : 0.f;
+        scalars[0] = surrogate + penalty - beta_entropy * entropy;
+        scalars[1] = kl_mean;
+        scalars[2] = entropy;
+        scalars[3] = r * inv_b;
+        scalars[4] = surrogate;
+    }
+}
+
+// AdditiveNoise.get_action([mean, std]) (exploration_policies/additive_noise.py:84-103) for the PPO actor:
+// std = exp(logstd) (the head's policy_std output, no eps); actions = (double) mean + (double) std * n, one multiply
+// and one add each rounded on its own, which is numpy's normal(mean, std) on the draws n.
+__global__ void __launch_bounds__(256) ppo_gaussian_act_kernel(const float* __restrict__ mean,
+                                                               const float* __restrict__ logstd, int64_t n, int A,
+                                                               const double* __restrict__ normals,
+                                                               double* __restrict__ actions, float* __restrict__ stds) {
+    for (int64_t k = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; k < n; k += (int64_t)gridDim.x * blockDim.x) {
+        const float std = expf(logstd[k % A]);
+        if (stds) stds[k] = std;
+        if (normals) actions[k] = __dadd_rn((double)mean[k], __dmul_rn((double)std, normals[k]));
+    }
+}
+
 }  // namespace cb200
 
 using namespace cb200;
@@ -805,6 +935,33 @@ int cb200_ppo_continuous_head(const float* mu, const float* logstd, const float*
     CB200_CHECK_ARG(batch > 0 && action_dim > 0 && action_dim <= kMaxActionDim, "bad shape (action_dim <= 32)");
     CB200_LAUNCH(ppo_continuous_head_kernel, 1, 256, 0, as_stream(stream), mu, logstd, actions, old_mu, old_logstd,
                  advantages, batch, action_dim, clip_eps, beta_entropy, d_mu, d_logstd, scalars);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_ppo_kl_head(const float* mu, const float* logstd, const float* actions, const float* old_mu,
+                      const float* old_logstd, const float* advantages, int64_t batch, int32_t action_dim,
+                      const float* kl_coef, float kl_cutoff, float high_kl_penalty, int32_t use_kl, float beta_entropy,
+                      float* d_mu, float* d_logstd, float* scalars, void* stream) {
+    CB200_CHECK_ARG(mu && logstd && actions && old_mu && old_logstd && advantages && d_mu && d_logstd, "null pointer");
+    CB200_CHECK_ARG(batch > 0 && action_dim > 0 && action_dim <= kMaxActionDim, "bad shape (action_dim <= 32)");
+    CB200_CHECK_ARG(!use_kl || kl_coef, "use_kl needs the device KL coefficient");
+    CB200_LAUNCH(ppo_kl_head_kernel, 1, kPpoKlThreads, 0, as_stream(stream), mu, logstd, actions, old_mu, old_logstd,
+                 advantages, batch, action_dim, kl_coef, kl_cutoff, high_kl_penalty, use_kl ? 1 : 0, beta_entropy,
+                 d_mu, d_logstd, scalars);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_ppo_gaussian_act(const float* mean, const float* logstd, int64_t envs, int32_t action_dim,
+                           const double* normals, double* actions, float* stds, void* stream) {
+    CB200_CHECK_ARG(mean && logstd && envs > 0 && action_dim > 0 && action_dim <= kMaxActionDim, "bad arguments");
+    CB200_CHECK_ARG(!normals || actions, "normals need actions");
+    const int64_t n = envs * action_dim;
+    int64_t grid = (n + 255) / 256;
+    if (grid > (int64_t)sm_count() * 8) grid = (int64_t)sm_count() * 8;
+    CB200_LAUNCH(ppo_gaussian_act_kernel, (unsigned)grid, 256, 0, as_stream(stream), mean, logstd, n, action_dim,
+                 normals, actions, stds);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

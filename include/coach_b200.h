@@ -811,6 +811,27 @@ int cb200_ppo_continuous_head(const float* mu, const float* logstd, const float*
                               float clip_eps, float beta_entropy, float* d_mu, float* d_logstd, float* scalars,
                               void* stream);
 
+/* PPOHead for continuous actions with the KL penalty and no clipping (heads/ppo_head.py:64-97 with
+ * clip_likelihood_ratio_using_epsilon None; agents/ppo_agent.py): the Gaussian terms of cb200_ppo_continuous_head and
+ *   KLbar = mean_i KL_i(old || new)
+ *   L     = -mean_i(ratio_i * A_i) + use_kl * (k * KLbar + high_kl_penalty * max(0, KLbar - kl_cutoff)^2) - beta * H
+ * (the two KL terms are the head's regularizations, :68-72; kl_cutoff = 2 * target_kl_divergence).  kl_coef is a
+ * DEVICE fp32 scalar k, read at run time, so a captured CUDA graph follows coefficient updates; it may be NULL when
+ * use_kl == 0.  Outputs d(L)/d(mu) [batch, action_dim], d(L)/d(logstd) [action_dim] and optional scalars[5] =
+ * {loss, KLbar, entropy, mean ratio, surrogate -mean(ratio * A)}.  One CTA with fixed-order reductions: repeat calls
+ * give identical bits.  1 <= action_dim <= 32, batch >= 1. */
+int cb200_ppo_kl_head(const float* mu, const float* logstd, const float* actions, const float* old_mu,
+                      const float* old_logstd, const float* advantages, int64_t batch, int32_t action_dim,
+                      const float* kl_coef, float kl_cutoff, float high_kl_penalty, int32_t use_kl, float beta_entropy,
+                      float* d_mu, float* d_logstd, float* scalars, void* stream);
+
+/* AdditiveNoise.get_action([mean, std]) of the PPO actor (exploration_policies/additive_noise.py:84-103):
+ * stds [envs, action_dim] = exp(logstd) in fp32 (optional); with normals [envs, action_dim] (np.random.standard_normal,
+ * what successive np.random.normal calls draw): actions = (double) mean + (double) std * n, multiply and add each
+ * rounded on its own (numpy's normal).  normals NULL: only stds are written (evaluation acts on the mean). */
+int cb200_ppo_gaussian_act(const float* mean, const float* logstd, int64_t envs, int32_t action_dim,
+                           const double* normals, double* actions, float* stds, void* stream);
+
 /* dst[c][i, :] = src[c][idx[*offset + i], :] for i < n (idx == NULL: rows *offset + i).  `offset` is a DEVICE scalar
  * so that the launch is identical for every minibatch of an epoch (CUDA-graph replay; only *offset changes).
  * Minibatch slicing of clipped_ppo_agent.py:232-265 after batch.shuffle(). */
