@@ -251,6 +251,8 @@ PROTOTYPES = {
                                   c_void_p]),
     "cb200_ppo_gaussian_act": (c_int, [c_void_p, c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p, c_void_p,
                                        c_void_p]),
+    "cb200_ppo_categorical_head": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_i64, ctypes.c_int32, c_float,
+                                           c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
     "cb200_gather_at": (c_int, [ctypes.POINTER(Column), c_int, c_void_p, c_void_p, c_i64, c_void_p]),
     "cb200_f64_to_f32": (c_int, [c_void_p, c_i64, c_void_p, c_void_p]),
     "cb200_sac_policy_sample": (c_int, [c_void_p, c_void_p, c_i64, ctypes.c_int32, c_void_p, c_void_p, c_void_p,

@@ -16,6 +16,17 @@ global norm -> Adam with device-side step state -> cursor += B) has launch param
 captured once in a CUDA graph and replayed for every minibatch of every epoch: 0 host work per minibatch.
 The old policy's mean is evaluated once per training phase for the whole rollout (the target network is frozen during
 ``train_network`` -- the reference recomputes identical values every minibatch, clipped_ppo_agent.py:238-240 TODO-perf).
+
+Discrete actions (``num_actions``; heads/ppo_head.py:100-116): the policy net ends in Dense(A) ``policy_fc`` (glorot,
+zero bias, no log-std) and the head is cb200_ppo_categorical_head.  The old policy is the target network's softmax over
+the rollout, once per phase.  The clip rescaler (the clipping schedule's value) lives in device memory, written at the
+start of each phase, so the rollout columns, the permutation and the captured minibatch graph persist across phases: the
+graph is captured once.  The continuous path keeps its epsilon as a launch argument and captures its graph per phase.
+
+Acting (clipped_ppo_agent.py:346-354): the pre-network filter without a statistics update, the policy net on the
+device, then Categorical (cb200_policy_act: np.random.choice on host uniforms, or the first argmax in evaluation) or
+AdditiveNoise on [mean, exp(log std)] (cb200_ppo_gaussian_act); the clipping schedule steps once per environment in
+training and evaluation, as the reference steps it in every choose_action.
 """
 import random
 
@@ -23,14 +34,20 @@ import numpy as np
 import torch
 
 from coach_b200 import _lib, parallel, rl_math
+from coach_b200.agents.actor_critic_agent import CategoricalParameters
 from coach_b200.architectures.layers import Dense, Workspace
 from coach_b200.architectures.network import ParamStore, Sequential
 from coach_b200.base_parameters import AgentParameters, AlgorithmParameters, EnvironmentSteps, NetworkParameters
 from coach_b200.core_types import DeviceBatch
+from coach_b200.exploration_policies.additive_noise import AdditiveNoiseParameters
 from coach_b200.filters.filter import InputFilter, ObservationNormalizationFilter
 from coach_b200.memories.episodic_experience_replay import EpisodicExperienceReplayParameters
 from coach_b200.schedules import ConstantSchedule
-from coach_b200.utils import dynamic_import_and_instantiate_module_from_params
+from coach_b200.utils import dynamic_import_and_instantiate_module_from_params, graph_capture
+
+# discrete actions: the categorical softmax and draw of cb200_policy_act (acting and the old policy) take 1 .. 18 actions,
+# Atari's full action set; cb200_ppo_categorical_head itself takes up to 32
+MAX_DISCRETE_ACTIONS = 18
 
 
 class ClippedPPONetworkParameters(NetworkParameters):
@@ -68,6 +85,8 @@ class ClippedPPOAgentParameters(AgentParameters):
     def __init__(self):
         super().__init__(algorithm=ClippedPPOAlgorithmParameters(), memory=EpisodicExperienceReplayParameters(),
                          networks={"main": ClippedPPONetworkParameters()})
+        self.exploration = {"DiscreteActionSpace": CategoricalParameters(),
+                            "BoxActionSpace": AdditiveNoiseParameters()}
         self.pre_network_filter = InputFilter()
         self.pre_network_filter.add_observation_filter('observation', 'normalize_observation',
                                                        ObservationNormalizationFilter(name='normalize_observation'))
@@ -80,21 +99,26 @@ class ClippedPPOAgentParameters(AgentParameters):
 class PPONetworkDef(object):
     """flat parameter layout of the two sub-networks (general_network.py:244-349 creation order)"""
 
-    def __init__(self, device, obs_dim, action_dim, hidden=64):
+    def __init__(self, device, obs_dim, action_dim, hidden=64, discrete=False):
+        """discrete: the policy net ends in the logits Dense(action_dim) (policy_fc) and has no log-std variable"""
         self.device = torch.device(device)
         self.D, self.A, self.Hd = int(obs_dim), int(action_dim), int(hidden)
+        self.discrete = bool(discrete)
         s = self.store = ParamStore(self.device)
         self.v_seq = Sequential([Dense(self.D, hidden, "tanh"), Dense(hidden, hidden, "tanh"), Dense(hidden, 1, None)],
                                 s, "main/online/network_0")
         s.add("main/online/network_0/gradients_from_head_0-0_rescalers", ())
         self.p_seq = Sequential([Dense(self.D, hidden, "tanh"), Dense(hidden, hidden, "tanh"),
                                  Dense(hidden, self.A, None)], s, "main/online/network_1")
-        self.logstd_name = s.add("main/online/network_1/ppo_head_0/policy_log_std", (self.A,))
+        self.logstd_name = None if self.discrete else \
+            s.add("main/online/network_1/ppo_head_0/policy_log_std", (self.A,))
         s.add("main/online/network_1/gradients_from_head_1-0_rescalers", ())
         s.finalize()
 
     def init(self, generator=None):
         self.store.init_glorot(generator)
+        if self.discrete:
+            return                                  # policy_fc: TF's default glorot kernel and zero bias (:109)
         self.store.view(self.store.theta, self.logstd_name).zero_()          # np.zeros((1, num_actions)), :129-133
         # policy mean layer: normalized_columns_initializer(0.01) (ppo_head.py:121, head.py:28-33)
         name = self.p_seq.names[2][0]
@@ -104,11 +128,32 @@ class PPONetworkDef(object):
 
 
 class ClippedPPOAgent(object):
-    def __init__(self, agent_parameters, parent=None, observation_dim=None, action_dim=None, device=None, seed=None):
+    def __init__(self, agent_parameters, parent=None, observation_dim=None, action_dim=None, device=None, seed=None,
+                 num_actions=None, action_low=None, action_high=None):
+        """num_actions: a discrete action space of that many actions; action_dim: a Box action space of that many
+        dimensions.  Give exactly one.  action_low / action_high: the Box bounds (scalars or per dimension), needed only
+        to act (AdditiveNoise refuses unbounded actions)."""
         self.ap = agent_parameters
+        # ---- refusals, before anything touches the GPU ----
+        if (num_actions is None) == (action_dim is None):
+            raise ValueError("give exactly one of num_actions (discrete actions) or action_dim (continuous actions)")
+        self.discrete = num_actions is not None
+        if self.discrete:
+            if not 1 <= int(num_actions) <= MAX_DISCRETE_ACTIONS:
+                raise ValueError("discrete ClippedPPO takes 1 .. %d actions (the categorical acting and softmax code), "
+                                 "got %d" % (MAX_DISCRETE_ACTIONS, num_actions))
+            if parallel.world()[1] > 1:
+                raise ValueError("discrete ClippedPPO runs on one rank")
+        self.action_low = self.action_high = None
+        if not self.discrete and action_low is not None and action_high is not None:
+            self.action_low = np.broadcast_to(np.asarray(action_low, dtype=np.float64), (int(action_dim),))
+            self.action_high = np.broadcast_to(np.asarray(action_high, dtype=np.float64), (int(action_dim),))
+        ex = getattr(self.ap, "exploration", None)
+        box = ex.get("BoxActionSpace") if isinstance(ex, dict) else ex
+        self.noise_schedule = None if self.discrete else getattr(box, "noise_schedule", None)
         self.lib = _lib.load()
         self.device = torch.device(device if device is not None else "cuda")
-        self.D, self.A = int(observation_dim), int(action_dim)
+        self.D, self.A = int(observation_dim), int(num_actions if self.discrete else action_dim)
         net_p = self.ap.network_wrappers["main"]
         self.B = int(net_p.batch_size)
         self.memory = dynamic_import_and_instantiate_module_from_params(
@@ -120,17 +165,23 @@ class ClippedPPOAgent(object):
                 for f in flt.values():
                     if hasattr(f, "set_shape"):
                         f.set_shape([self.D])
-        self.net = PPONetworkDef(self.device, self.D, self.A, getattr(net_p, "hidden_units", 64))
+        self.net = PPONetworkDef(self.device, self.D, self.A, getattr(net_p, "hidden_units", 64), self.discrete)
         gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
         self.net.init(gen)
         st = self.net.store
         self.theta_target = st.new_buffer()
-        self.ws = Workspace(self.device)
+        # the captured minibatch step holds its workspace's pointer; rollout-sized and acting passes, which may grow
+        # theirs, use another
+        self.ws, self.ws_rollout = Workspace(self.device), Workspace(self.device)
         dev, B = self.device, self.B
         f32 = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)     # noqa: E731
         # persistent minibatch buffers
-        self.mb = dict(states=f32(B, self.D), actions=f32(B, self.A), advantages=f32(B), value_targets=f32(B, 1),
-                       old_mu=f32(B, self.A))
+        if self.discrete:
+            self.mb = dict(states=f32(B, self.D), actions=torch.zeros(B, dtype=torch.int64, device=dev),
+                           advantages=f32(B), value_targets=f32(B, 1), old_probs=f32(B, self.A))
+        else:
+            self.mb = dict(states=f32(B, self.D), actions=f32(B, self.A), advantages=f32(B), value_targets=f32(B, 1),
+                           old_mu=f32(B, self.A))
         self.v_inst = self.net.v_seq.instantiate(self.lib, self.ws, B, self.mb["states"], st.theta, st.grad,
                                                  train=True)
         self.p_inst = self.net.p_seq.instantiate(self.lib, self.ws, B, self.mb["states"], st.theta, st.grad,
@@ -141,9 +192,15 @@ class ClippedPPOAgent(object):
         self.adam_state = torch.tensor([net_p.adam_optimizer_beta1, net_p.adam_optimizer_beta2], dtype=torch.float32,
                                        device=dev)
         self.cursor = torch.zeros(1, dtype=torch.int64, device=dev)
+        # the clipping schedule's value as the discrete head reads it (fp32, written at the start of every phase)
+        self.clip_rescaler = f32(1)
         self._graph = None
         self._graph_key = None
+        self.graph_captures = 0
+        self._rows = None          # discrete: persistent rollout-sized training columns (capacity, dict, argmax scratch)
+        self._perm = None          # discrete: persistent permutation of the rollout rows
         self._full = {}            # rollout-sized forward instances, keyed by N
+        self._act = {}             # acting buffers, keyed by the number of environments
         self.training_iteration = 0
         self.total_steps_counter = 0
         self.last_training_phase_step = 0
@@ -164,8 +221,8 @@ class ClippedPPOAgent(object):
         if N not in self._full:
             st = self.net.store
             x = torch.zeros((N, self.D), dtype=torch.float32, device=self.device)
-            v = self.net.v_seq.instantiate(self.lib, self.ws, N, x, st.theta)
-            p_old = self.net.p_seq.instantiate(self.lib, self.ws, N, x, self.theta_target)
+            v = self.net.v_seq.instantiate(self.lib, self.ws_rollout, N, x, st.theta)
+            p_old = self.net.p_seq.instantiate(self.lib, self.ws_rollout, N, x, self.theta_target)
             self._full = {N: (x, v, p_old)}           # keep only the latest size
         return self._full[N]
 
@@ -186,7 +243,8 @@ class ClippedPPOAgent(object):
         alg, net_p = self.ap.algorithm, self.ap.network_wrappers["main"]
         arr, cnt = _lib.make_columns([(data[k].data_ptr(), self.mb[k].data_ptr(),
                                        self.mb[k].element_size() * int(np.prod(self.mb[k].shape[1:])))
-                                      for k in ("states", "actions", "advantages", "value_targets", "old_mu")])
+                                      for k in ("states", "actions", "advantages", "value_targets",
+                                                "old_probs" if self.discrete else "old_mu")])
         _lib.check(lib.cb200_gather_at(arr, cnt, perm.data_ptr(), self.cursor.data_ptr(), self.B, st))
         v = self.v_inst.forward()
         mu = self.p_inst.forward()
@@ -194,15 +252,22 @@ class ClippedPPOAgent(object):
         _lib.check(lib.cb200_regression_head_loss_grad(v.data_ptr(), self.mb["value_targets"].data_ptr(), None,
                                                        self.B, 1, 0, 1.0, self.v_inst.d_out.data_ptr(),
                                                        self.v_loss.data_ptr(), st))
-        clip_eps = float(alg.clip_likelihood_ratio_using_epsilon) * float(alg.clipping_decay_schedule.current_value)
-        logstd = store.view(store.theta, self.net.logstd_name)
-        old_logstd = store.view(self.theta_target, self.net.logstd_name)
-        d_logstd = store.view(store.grad, self.net.logstd_name)
-        _lib.check(lib.cb200_ppo_continuous_head(mu.data_ptr(), logstd.data_ptr(), self.mb["actions"].data_ptr(),
-                                                 self.mb["old_mu"].data_ptr(), old_logstd.data_ptr(),
-                                                 self.mb["advantages"].data_ptr(), self.B, self.A, clip_eps,
-                                                 float(alg.beta_entropy), self.p_inst.d_out.data_ptr(),
-                                                 d_logstd.data_ptr(), self.scalars.data_ptr(), st))
+        if self.discrete:
+            _lib.check(lib.cb200_ppo_categorical_head(mu.data_ptr(), self.mb["actions"].data_ptr(),
+                                                      self.mb["old_probs"].data_ptr(), self.mb["advantages"].data_ptr(),
+                                                      self.B, self.A, float(alg.clip_likelihood_ratio_using_epsilon),
+                                                      self.clip_rescaler.data_ptr(), float(alg.beta_entropy),
+                                                      self.p_inst.d_out.data_ptr(), self.scalars.data_ptr(), st))
+        else:
+            clip_eps = float(alg.clip_likelihood_ratio_using_epsilon) * float(alg.clipping_decay_schedule.current_value)
+            logstd = store.view(store.theta, self.net.logstd_name)
+            old_logstd = store.view(self.theta_target, self.net.logstd_name)
+            d_logstd = store.view(store.grad, self.net.logstd_name)
+            _lib.check(lib.cb200_ppo_continuous_head(mu.data_ptr(), logstd.data_ptr(), self.mb["actions"].data_ptr(),
+                                                     self.mb["old_mu"].data_ptr(), old_logstd.data_ptr(),
+                                                     self.mb["advantages"].data_ptr(), self.B, self.A, clip_eps,
+                                                     float(alg.beta_entropy), self.p_inst.d_out.data_ptr(),
+                                                     d_logstd.data_ptr(), self.scalars.data_ptr(), st))
         self.v_inst.backward()
         self.p_inst.backward()
         n = store.size
@@ -222,18 +287,31 @@ class ClippedPPOAgent(object):
 
     def train_network(self, data, n_rows, epochs):
         """clipped_ppo_agent.py:209-308.  data: dict of rollout-sized CUDA tensors (states, actions, advantages,
-        value_targets, old_mu).  Returns the mean [value loss, policy loss] of the last epoch as device tensors."""
+        value_targets, and old_mu, or old_probs for discrete actions: int64 actions [N] and the old policy's
+        probabilities [N, A]).  Returns the mean [value loss, policy loss] of the last epoch as device tensors."""
         B = self.B
         n_full = n_rows // B
         if n_rows % B:
             raise ValueError("the rollout length (%d) must be a multiple of the batch size (%d)" % (n_rows, B))
-        perm_host = torch.zeros(n_rows, dtype=torch.int64, pin_memory=self.device.type == "cuda")
-        perm = torch.zeros(n_rows, dtype=torch.int64, device=self.device)
-        key = (tuple(t.data_ptr() for t in data.values()), perm.data_ptr(), n_rows,
-               float(self.ap.algorithm.clipping_decay_schedule.current_value))
+        # one pinned row per epoch: an epoch's asynchronous copy may still be queued when the host shuffles the next
+        perm_host = torch.zeros((epochs, n_rows), dtype=torch.int64, pin_memory=self.device.type == "cuda")
+        if self.discrete:
+            # the clipping schedule reaches the head through the device rescaler, so the key leaves it out and one
+            # graph serves every phase that trains on the same columns
+            if self._perm is None or self._perm.numel() < n_rows:
+                self._perm = torch.zeros(n_rows, dtype=torch.int64, device=self.device)
+            perm = self._perm
+            key = (tuple(t.data_ptr() for t in data.values()), perm.data_ptr())
+            self.clip_rescaler.fill_(float(self.ap.algorithm.clipping_decay_schedule.current_value))
+        else:
+            perm = torch.zeros(n_rows, dtype=torch.int64, device=self.device)
+            key = (tuple(t.data_ptr() for t in data.values()), perm.data_ptr(), n_rows,
+                   float(self.ap.algorithm.clipping_decay_schedule.current_value))
         world = parallel.world()[1]
         graphable = self.use_cuda_graph and self.device.type == "cuda" and world == 1
-        if graphable:
+        if graphable and self.discrete and key == self._graph_key:
+            graph = self._graph
+        elif graphable:
             # warm-up launch outside capture (lazy module loading), then capture once.  The warm-up gathers at the
             # cursor, which a previous phase left at its rollout's end: start it at row 0, inside this permutation.
             self.cursor.zero_()
@@ -243,16 +321,18 @@ class ClippedPPOAgent(object):
                 self._snapshot_then_restore(lambda: self._minibatch_kernels(data, perm, n_rows))
             torch.cuda.current_stream().wait_stream(side)
             graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
+            with graph_capture(graph):
                 self._minibatch_kernels(data, perm, n_rows)
             self._restore_snapshot()
+            self._graph, self._graph_key = graph, key
+            self.graph_captures += 1
         order = list(range(n_rows))
         v_acc = torch.zeros(1, dtype=torch.float32, device=self.device)
         p_acc = torch.zeros(1, dtype=torch.float32, device=self.device)
         for epoch in range(epochs):
             random.shuffle(order)                                   # batch.shuffle(), core_types.py:452-468
-            perm_host.copy_(torch.tensor(order, dtype=torch.int64))
-            perm.copy_(perm_host, non_blocking=True)
+            perm_host[epoch].copy_(torch.tensor(order, dtype=torch.int64))
+            perm[:n_rows].copy_(perm_host[epoch], non_blocking=True)
             self.cursor.zero_()
             v_acc.zero_()
             p_acc.zero_()
@@ -304,6 +384,11 @@ class ClippedPPOAgent(object):
             batch = self.pre_network_filter.filter(batch, deep_copy=False,
                                                    update_internal_state=alg.update_pre_network_filters_state_on_train)
         states = batch.states(["observation"])["observation"].to(torch.float32).contiguous()
+        if self.discrete:
+            self._train_discrete(batch, states)
+            self.memory.clean()
+            self.training_iteration += 1
+            return None
         actions = batch.actions().to(torch.float32).reshape(batch.size, self.A).contiguous()
         for _ in range(alg.num_consecutive_training_steps):
             self.sync()
@@ -326,3 +411,120 @@ class ClippedPPOAgent(object):
         self.memory.clean()                                            # post_training_commands :310-312
         self.training_iteration += 1
         return None
+
+    def _training_rows(self, n_rows):
+        """discrete: the persistent training columns and the scratch argmax of the old-policy softmax, grown when a
+        phase trains on more rows (the captured graph holds their pointers)"""
+        if self._rows is None or self._rows[0] < n_rows:
+            f32 = lambda *s: torch.zeros(s, dtype=torch.float32, device=self.device)      # noqa: E731
+            cols = dict(states=f32(n_rows, self.D), actions=torch.zeros(n_rows, dtype=torch.int64, device=self.device),
+                        advantages=f32(n_rows), value_targets=f32(n_rows, 1), old_probs=f32(n_rows, self.A))
+            self._rows = (n_rows, cols, torch.zeros(n_rows, dtype=torch.int64, device=self.device))
+        return self._rows[1], self._rows[2]
+
+    def _train_discrete(self, batch, states):
+        """the discrete branch of train(): actions stay int64, the old policy is the target network's softmax"""
+        alg = self.ap.algorithm
+        actions = batch.actions().reshape(batch.size).to(torch.int64)
+        for _ in range(alg.num_consecutive_training_steps):
+            self.sync()
+            adv, tgt, n_valid = self.fill_advantages(states, batch.rewards(), batch.game_overs())
+            n_rows = batch.size
+            if alg.truncate_dataset_to_playing_steps:
+                n_rows = min(n_rows, alg.num_consecutive_playing_steps.num_steps)
+            if n_rows < self.B:
+                raise ValueError("the rollout holds %d transitions, fewer than one minibatch of %d: nothing to train on "
+                                 "(the reference would train on one partial minibatch)" % (n_rows, self.B))
+            n_rows = (n_rows // self.B) * self.B
+            cols, argmax = self._training_rows(n_rows)
+            _, _, p_old = self._full_instances(batch.size)
+            logits_old = p_old.forward()                               # frozen target network, whole rollout at once
+            # the old policy's probabilities: the categorical softmax of the acting code (its argmax is not used)
+            _lib.check(self.lib.cb200_policy_act(logits_old.data_ptr(), n_rows, self.A, 0, None, None, None,
+                                                 argmax.data_ptr(), cols["old_probs"].data_ptr(), None, None,
+                                                 _lib.current_stream()))
+            cols["states"][:n_rows].copy_(states[:n_rows])
+            cols["actions"][:n_rows].copy_(actions[:n_rows])
+            cols["advantages"][:n_rows].copy_(adv[:n_rows])
+            cols["value_targets"][:n_rows].copy_(tgt[:n_rows].reshape(-1, 1))
+            self.train_network(cols, n_rows, alg.optimization_epochs)
+
+    # ---- acting ------------------------------------------------------------------------------------------------------
+    def _act_buffers(self, E):
+        if E not in self._act:
+            dev, pin = self.device, self.device.type == "cuda"
+            x = torch.zeros((E, self.D), dtype=torch.float32, device=dev)
+            inst = self.net.p_seq.instantiate(self.lib, self.ws_rollout, E, x, self.net.store.theta)
+            shape = (E,) if self.discrete else (E, self.A)
+            self._act = {E: dict(x=x, inst=inst, actions=torch.zeros(E, dtype=torch.int64, device=dev),
+                                 probs=torch.zeros((E, self.A), dtype=torch.float32, device=dev),
+                                 cont=torch.zeros((E, self.A), dtype=torch.float64, device=dev),
+                                 stds=torch.zeros((E, self.A), dtype=torch.float32, device=dev),
+                                 d_dev=torch.zeros(shape, dtype=torch.float64, device=dev),
+                                 d_host=torch.zeros(shape, dtype=torch.float64, pin_memory=pin))}
+        return self._act[E]
+
+    def choose_actions(self, states, evaluation=False, uniforms=None, normals=None):
+        """clipped_ppo_agent.py:346-354 and policy_optimization_agent.py:160-185 for E environments.  The states pass
+        the pre-network filter without a statistics update (update_pre_network_filters_state_on_inference False), and
+        the clipping schedule is stepped E times, in training and evaluation.
+        Discrete: Categorical.get_action on softmax(logits): np.random.choice(A, p) on ``uniforms`` [E] (default
+        np.random.random_sample(E), what E successive choice calls draw) in training, the first argmax in evaluation.
+        Returns (actions int64 [E], probabilities float32 [E, A]).
+        Continuous: AdditiveNoise.get_action([mean, std]), std = exp(policy_log_std): np.random.normal(mean, std) =
+        (double) mean + (double) std * n on ``normals`` [E, A] (default np.random.standard_normal((E, A))) in training,
+        stepping the noise schedule E times; the fp32 mean in evaluation.  Returns (actions [E, A]: float64 in
+        training, float32 in evaluation, means float32 [E, A], stds float32 [E, A])."""
+        if not self.discrete and (self.action_low is None or not (np.all(np.isfinite(self.action_low)) and
+                                                                  np.all(np.isfinite(self.action_high)))):
+            raise ValueError("Additive noise exploration requires bounded actions: build the agent with finite "
+                             "action_low / action_high")
+        alg, A = self.ap.algorithm, self.A
+        s = torch.as_tensor(np.asarray(states, dtype=np.float32)).reshape(-1, self.D)
+        E = int(s.shape[0])
+        buf = self._act_buffers(E)
+        x = s.to(self.device)
+        if self.pre_network_filter is not None:
+            for flt in self.pre_network_filter._observation_filters.values():
+                for f in flt.values():
+                    x = f.filter(x, update_internal_state=alg.update_pre_network_filters_state_on_inference)
+        buf["x"].copy_(x)
+        z = buf["inst"].forward()
+        for _ in range(E):
+            alg.clipping_decay_schedule.step()
+        d_ptr = None
+        if not evaluation:
+            if self.discrete:
+                d = np.random.random_sample(E) if uniforms is None else np.asarray(uniforms, dtype=np.float64)
+            else:
+                d = np.random.standard_normal((E, A)) if normals is None else np.asarray(normals, dtype=np.float64)
+                for _ in range(E):
+                    self.noise_schedule.step()
+            torch.cuda.current_stream().synchronize()            # the previous call's copy has left the staging
+            buf["d_host"].numpy()[...] = d.reshape(buf["d_host"].shape)
+            buf["d_dev"].copy_(buf["d_host"], non_blocking=True)
+            d_ptr = buf["d_dev"].data_ptr()
+        st = _lib.current_stream()
+        if self.discrete:
+            _lib.check(self.lib.cb200_policy_act(z.data_ptr(), E, A, 0, None, d_ptr, None, buf["actions"].data_ptr(),
+                                                 buf["probs"].data_ptr(), None, None, st))
+            return buf["actions"].cpu().numpy(), buf["probs"].cpu().numpy()
+        logstd = self.net.store.view(self.net.store.theta, self.net.logstd_name)
+        _lib.check(self.lib.cb200_ppo_gaussian_act(z.data_ptr(), logstd.data_ptr(), E, A, d_ptr,
+                                                   buf["cont"].data_ptr(), buf["stds"].data_ptr(), st))
+        means, stds = z.cpu().numpy().copy(), buf["stds"].cpu().numpy()
+        return (means.copy() if evaluation else buf["cont"].cpu().numpy()), means, stds
+
+    # ---- checkpoint host state ---------------------------------------------------------------------------------------
+    def checkpoint_state(self):
+        """the clipping schedule's value, and the noise schedule's for continuous actions (the networks go through the
+        ClippedPPO checkpoint item)"""
+        state = dict(clipping=float(self.ap.algorithm.clipping_decay_schedule.current_value))
+        if not self.discrete:
+            state["noise"] = float(self.noise_schedule.current_value)
+        return state
+
+    def restore_checkpoint_state(self, state):
+        self.ap.algorithm.clipping_decay_schedule.current_value = state["clipping"]
+        if "noise" in state:
+            self.noise_schedule.current_value = state["noise"]

@@ -26,7 +26,7 @@ from coach_b200.architectures.network import ParamStore, Sequential
 from coach_b200.base_parameters import (AgentParameters, AlgorithmParameters, EnvironmentSteps, NetworkParameters,
                                         TrainingSteps)
 from coach_b200.memories.episodic_experience_replay import EpisodicExperienceReplayParameters
-from coach_b200.utils import dynamic_import_and_instantiate_module_from_params
+from coach_b200.utils import dynamic_import_and_instantiate_module_from_params, graph_capture
 
 RELU, TANH = 1, 2
 
@@ -122,7 +122,7 @@ class GraphedKernels(object):
             torch.cuda.synchronize()
             c0 = lib.cb200_launch_count()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
+            with graph_capture(g):
                 self.fn()
             self.launches = int(lib.cb200_launch_count() - c0)
             self.graph = g

@@ -26,7 +26,7 @@ from coach_b200.base_parameters import (AgentParameters, AlgorithmParameters, En
                                         NetworkParameters, TrainingSteps)
 from coach_b200.memories.experience_replay import ExperienceReplayParameters
 from coach_b200.memories.prioritized_experience_replay import PrioritizedExperienceReplay
-from coach_b200.utils import dynamic_import_and_instantiate_module_from_params
+from coach_b200.utils import dynamic_import_and_instantiate_module_from_params, graph_capture
 from coach_b200 import parallel
 
 
@@ -480,7 +480,7 @@ class DQNAgent(object):
         if len(self._graphs) == k:
             c0 = self.lib.cb200_launch_count()
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
+            with graph_capture(g):
                 part(*args)
             self._graphs.append((g, int(self.lib.cb200_launch_count() - c0)))
         g, n = self._graphs[k]

@@ -75,6 +75,8 @@ def _load_into(path, t, rows=None, chunk_bytes=1 << 28):
     if dst.dim() == 0:
         dst.fill_(arr.item())
         return
+    if dst.numel() == 0:                   # an empty replay (ClippedPPO right after a training phase) saves no rows
+        return
     per = max(1, int(chunk_bytes // max(1, dst[0].numel() * dst.element_size())))
     for lo in range(0, dst.shape[0], per):
         dst[lo:lo + per].copy_(torch.from_numpy(np.ascontiguousarray(arr[lo:lo + per])))

@@ -861,6 +861,99 @@ __global__ void __launch_bounds__(256) ppo_gaussian_act_kernel(const float* __re
     }
 }
 
+// =====================================================================================================================
+// PPOHead, discrete actions, clipped surrogate (heads/ppo_head.py:52-116).  TF 1.x's Categorical(probs = p) takes
+// logits = log p, so per row i, with p = softmax(z_i) and q_i the old policy's probabilities:
+//   log pi_j   = log_softmax(log p)_j = z_j - max z - log sum exp(z - max z)
+//   log pio_j  = log_softmax(log q)_j
+//   H_i        = -sum_j p_j log pi_j,   KL_i = sum_j softmax(log q)_j (log pio_j - log pi_j)  (0 where that weight is 0)
+//   ratio_i    = exp(log pi_a - log pio_a),  clipped to 1 -+ e,  e = fl32(clip_eps * rescaler)
+//   L          = -mean_i min(ratio_i A_i, clip(ratio_i) A_i)  -  beta * mean_i H_i
+//   dL/dz_ij   = -(1/B) dmin/dratio_i ratio_i (onehot(a_i)_j - p_j)  +  (beta/B) p_j (log pi_j + H_i)
+// A row whose action lies outside [0, A) has no surrogate term (nothing in the loss, ratio sums or gradient from it).
+// One CTA.  A warp owns a row at a time and lane j its action j (A <= 32); the per-row sums are xor-shuffle trees, so
+// every lane holds them bit for bit.  Each warp accumulates its rows in order and the warps' partials are summed in
+// warp order: no atomics, repeat calls and graph replays give identical bits.  The rescaler is read from device
+// memory so a captured graph follows a clipping schedule.
+// =====================================================================================================================
+constexpr int kPpoCatThreads = 1024;
+constexpr int kPpoCatWarps = kPpoCatThreads / 32;
+
+__global__ void __launch_bounds__(kPpoCatThreads) ppo_categorical_head_kernel(
+    const float* __restrict__ logits, const int64_t* __restrict__ actions, const float* __restrict__ old_probs,
+    const float* __restrict__ advantages, int64_t B, int A, float clip_eps, const float* __restrict__ clip_rescaler,
+    float beta_entropy, float* __restrict__ d_logits,
+    float* __restrict__ scalars /* [loss, KL(old||new), entropy, mean ratio, mean clipped ratio] */) {
+    __shared__ float part[5][kPpoCatWarps];              // per warp: surrogate min, KL, entropy, ratio, clipped ratio
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool on = lane < A;
+    const float inv_b = 1.0f / (float)B;
+    const float e = __fmul_rn(clip_eps, *clip_rescaler);      // TF: 1 +- eps * rescaler, the product in fp32
+    const float lo = 1.0f - e, hi = 1.0f + e;
+    const float ent_w = beta_entropy * inv_b;
+    float surr_acc = 0.f, kl_acc = 0.f, ent_acc = 0.f, ratio_acc = 0.f, cratio_acc = 0.f;
+    for (int64_t i = warp; i < B; i += kPpoCatWarps) {
+        const float z = on ? logits[i * A + lane] : -INFINITY;
+        const float m = warp_max(z);
+        const float ez = on ? expf(z - m) : 0.f;
+        const float s = warp_sum(ez);
+        const float p = ez / s;
+        const float lp = on ? (z - m) - logf(s) : 0.f;
+        const float lq = on ? logf(old_probs[i * A + lane]) : -INFINITY;
+        const float mq = warp_max(lq);
+        const float eq = on ? expf(lq - mq) : 0.f;
+        const float sq = warp_sum(eq);
+        const float qn = eq / sq;
+        const float lpo = on ? (lq - mq) - logf(sq) : 0.f;
+        const float H = -warp_sum(on ? p * lp : 0.f);
+        kl_acc += warp_sum(qn > 0.f ? qn * (lpo - lp) : 0.f);
+        ent_acc += H;
+        const int64_t a = actions[i];
+        const bool valid = a >= 0 && a < A;
+        const int ai = valid ? (int)a : 0;
+        const float lp_a = __shfl_sync(0xffffffffu, lp, ai), lpo_a = __shfl_sync(0xffffffffu, lpo, ai);
+        float dlogp = 0.f;                                    // dL/dlog pi_a
+        if (valid) {
+            const float ratio = expf(lp_a - lpo_a);
+            const float cl = fminf(fmaxf(ratio, lo), hi);
+            const float adv = advantages[i];
+            const float s1 = ratio * adv, s2 = cl * adv;
+            // tf.minimum passes the gradient to its first argument when s1 <= s2; clip_by_value passes it inside
+            // [lo, hi]
+            float ds_dratio;
+            if (s1 <= s2) ds_dratio = adv;
+            else ds_dratio = (ratio >= lo && ratio <= hi) ? adv : 0.f;
+            surr_acc += fminf(s1, s2);
+            ratio_acc += ratio;
+            cratio_acc += cl;
+            dlogp = -inv_b * ds_dratio * ratio;
+        }
+        if (on) {
+            const float onehot = (valid && lane == ai) ? 1.f : 0.f;
+            d_logits[i * A + lane] = dlogp * (onehot - p) + ent_w * p * (lp + H);
+        }
+    }
+    if (lane == 0) {
+        part[0][warp] = surr_acc;
+        part[1][warp] = kl_acc;
+        part[2][warp] = ent_acc;
+        part[3][warp] = ratio_acc;
+        part[4][warp] = cratio_acc;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && scalars) {
+        float t[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+        for (int w = 0; w < kPpoCatWarps; ++w)
+            for (int k = 0; k < 5; ++k) t[k] += part[k][w];
+        const float entropy = t[2] * inv_b;
+        scalars[0] = -t[0] * inv_b - beta_entropy * entropy;
+        scalars[1] = t[1] * inv_b;
+        scalars[2] = entropy;
+        scalars[3] = t[3] * inv_b;
+        scalars[4] = t[4] * inv_b;
+    }
+}
+
 }  // namespace cb200
 
 using namespace cb200;
@@ -949,6 +1042,18 @@ int cb200_ppo_kl_head(const float* mu, const float* logstd, const float* actions
     CB200_LAUNCH(ppo_kl_head_kernel, 1, kPpoKlThreads, 0, as_stream(stream), mu, logstd, actions, old_mu, old_logstd,
                  advantages, batch, action_dim, kl_coef, kl_cutoff, high_kl_penalty, use_kl ? 1 : 0, beta_entropy,
                  d_mu, d_logstd, scalars);
+    CB200_CHECK_LAUNCH();
+    return CB200_OK;
+}
+
+int cb200_ppo_categorical_head(const float* logits, const int64_t* actions, const float* old_probs,
+                               const float* advantages, int64_t batch, int32_t n_actions, float clip_eps,
+                               const float* clip_rescaler, float beta_entropy, float* d_logits, float* scalars,
+                               void* stream) {
+    CB200_CHECK_ARG(logits && actions && old_probs && advantages && clip_rescaler && d_logits, "null pointer");
+    CB200_CHECK_ARG(batch > 0 && n_actions > 0 && n_actions <= kMaxActionDim, "bad shape (1 <= n_actions <= 32)");
+    CB200_LAUNCH(ppo_categorical_head_kernel, 1, kPpoCatThreads, 0, as_stream(stream), logits, actions, old_probs,
+                 advantages, batch, n_actions, clip_eps, clip_rescaler, beta_entropy, d_logits, scalars);
     CB200_CHECK_LAUNCH();
     return CB200_OK;
 }

@@ -22,6 +22,7 @@ import numpy as np
 import torch
 
 from coach_b200 import _lib
+from coach_b200.utils import graph_capture
 
 COLUMNS = ("state", "next_state", "action", "reward", "game_over")
 
@@ -211,7 +212,7 @@ class LockstepSegments(object):
             if g is None:
                 c0 = self.lib.cb200_launch_count()
                 g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
+                with graph_capture(g):
                     step(B, gather)
                 g = self._graphs[B] = (g, int(self.lib.cb200_launch_count() - c0))
             g[0].replay()

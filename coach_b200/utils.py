@@ -1,8 +1,12 @@
 """Plugin loading the way Coach does it (rl_coach/utils.py:334-404): components are named by ``'module:Class'`` path
 strings carried by their Parameters object and instantiated with the intersection of constructor argument names and
 parameter attributes."""
+import contextlib
+import gc
 import importlib
 import inspect
+
+import torch
 
 
 def short_dynamic_import(module_path_and_attribute: str):
@@ -23,3 +27,20 @@ def dynamic_import_and_instantiate_module_from_params(module_parameters, path=No
         if k in ctor_args:
             kwargs[k] = v
     return cls(*positional_args, **kwargs)
+
+
+@contextlib.contextmanager
+def graph_capture(graph):
+    """``torch.cuda.graph(graph)`` with Python's cyclic garbage collector held off.  Agents are often reference cycles
+    (a graphed step holds a bound method of its agent), so pinned staging buffers of dead agents are freed only when
+    the collector runs; freeing a pinned block that served an asynchronous copy records a CUDA event on that copy's
+    stream, which invalidates a capture in progress.  Garbage is collected before the capture instead."""
+    gc.collect()
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(graph):
+            yield
+    finally:
+        if enabled:
+            gc.enable()

@@ -825,6 +825,24 @@ int cb200_ppo_kl_head(const float* mu, const float* logstd, const float* actions
                       const float* kl_coef, float kl_cutoff, float high_kl_penalty, int32_t use_kl, float beta_entropy,
                       float* d_mu, float* d_logstd, float* scalars, void* stream);
 
+/* PPOHead for discrete actions with the clipped surrogate (heads/ppo_head.py:52-116; agents/clipped_ppo_agent.py).
+ * logits [batch, n_actions] are the policy's last Dense outputs, p = softmax(logits); old_probs [batch, n_actions] the
+ * frozen target network's softmax.  TF 1.x's Categorical(probs = x) takes logits log x, so
+ *   log pi = log_softmax(log p), log pi_old = log_softmax(log old_probs), ratio = exp(log pi(a) - log pi_old(a)),
+ *   clipped to 1 -+ e with e = fl32(clip_eps * *clip_rescaler) (TF's fp32 product),
+ *   L = -mean_i min(ratio_i A_i, clip(ratio_i) A_i) - beta_entropy * mean_i H_i,  H_i = -sum_j p_j log pi_j.
+ * clip_rescaler is a DEVICE fp32 scalar read at run time, so one captured CUDA graph follows the clipping schedule.
+ * An action outside [0, n_actions) contributes no surrogate term: its row adds nothing to the loss's surrogate part,
+ * the ratio sums or the surrogate gradient (it still adds its entropy and KL terms, and every mean divides by batch).
+ * Outputs d(L)/d(logits) [batch, n_actions] and optional scalars[5] = {loss, mean KL(old||new), mean entropy,
+ * mean ratio, mean clipped ratio} (the signals of cb200_ppo_continuous_head, in its order); a KL term whose old
+ * probability is 0 counts as 0.  One CTA with fixed-order reductions: repeat calls give identical bits.
+ * 1 <= n_actions <= 32, batch >= 1; a bad argument returns an error and writes nothing. */
+int cb200_ppo_categorical_head(const float* logits, const int64_t* actions, const float* old_probs,
+                               const float* advantages, int64_t batch, int32_t n_actions, float clip_eps,
+                               const float* clip_rescaler, float beta_entropy, float* d_logits, float* scalars,
+                               void* stream);
+
 /* AdditiveNoise.get_action([mean, std]) of the PPO actor (exploration_policies/additive_noise.py:84-103):
  * stds [envs, action_dim] = exp(logstd) in fp32 (optional); with normals [envs, action_dim] (np.random.standard_normal,
  * what successive np.random.normal calls draw): actions = (double) mean + (double) std * n, multiply and add each
