@@ -9,19 +9,21 @@
 
 Network (presets/Mujoco_ClippedPPO.py:30-37, use_separate_networks_per_head): value net obs->64->64->1 and policy net
 obs->64->64->A, tanh, plus the state-independent ``policy_log_std`` variable; variables in TF creation order inside
-ONE flat buffer, so both sub-networks share a single gradient norm / Adam / all-reduce launch.
+ONE flat buffer, the network wrapper ``_Net`` (``main``: target copy, device-state Adam), so both sub-networks share a
+single gradient norm / Adam / all-reduce launch.
 
-The minibatch step (row gather at a device-side cursor -> value fwd/bwd -> policy fwd -> PPO head -> policy bwd ->
-global norm -> Adam with device-side step state -> cursor += B) has launch parameters that never change, so it is
-captured once in a CUDA graph and replayed for every minibatch of every epoch: 0 host work per minibatch.
-The old policy's mean is evaluated once per training phase for the whole rollout (the target network is frozen during
-``train_network`` -- the reference recomputes identical values every minibatch, clipped_ppo_agent.py:238-240 TODO-perf).
+Each phase evaluates the old policy once for the whole rollout (the target network is frozen during ``train_network``
+-- the reference recomputes identical values every minibatch, clipped_ppo_agent.py:238-240 TODO-perf) and stages the
+rollout into persistent training columns and a persistent permutation, grown only when a phase needs more rows.  The
+minibatch step (row gather through the permutation at a device-side cursor -> value fwd/bwd -> policy fwd -> PPO head ->
+policy bwd -> global norm -> Adam with device-side step state -> loss accumulators -> cursor += B) has launch parameters
+that never change, so it is a ``GraphedKernels``: captured once and replayed for every minibatch of every epoch and
+phase, 0 host work per minibatch, and rebuilt only when the columns grow or its clip epsilon changes.
 
 Discrete actions (``num_actions``; heads/ppo_head.py:100-116): the policy net ends in Dense(A) ``policy_fc`` (glorot,
-zero bias, no log-std) and the head is cb200_ppo_categorical_head.  The old policy is the target network's softmax over
-the rollout, once per phase.  The clip rescaler (the clipping schedule's value) lives in device memory, written at the
-start of each phase, so the rollout columns, the permutation and the captured minibatch graph persist across phases: the
-graph is captured once.  The continuous path keeps its epsilon as a launch argument and captures its graph per phase.
+zero bias, no log-std), the old policy is the target network's softmax and the head is cb200_ppo_categorical_head.  It
+reads the clipping schedule's value from a device rescaler written at the start of each phase, so one graph follows a
+moving schedule; the continuous head takes fp32(epsilon * value) as a launch argument, so a new value rebuilds its step.
 
 Acting (clipped_ppo_agent.py:346-354): the pre-network filter without a statistics update, the policy net on the
 device, then Categorical (cb200_policy_act: np.random.choice on host uniforms, or the first argmax in evaluation) or
@@ -35,6 +37,7 @@ import torch
 
 from coach_b200 import _lib, parallel, rl_math
 from coach_b200.agents.actor_critic_agent import CategoricalParameters
+from coach_b200.agents.ddpg_agent import GraphedKernels, _Net
 from coach_b200.architectures.layers import Dense, Workspace
 from coach_b200.architectures.network import ParamStore, Sequential
 from coach_b200.base_parameters import AgentParameters, AlgorithmParameters, EnvironmentSteps, NetworkParameters
@@ -43,7 +46,7 @@ from coach_b200.exploration_policies.additive_noise import AdditiveNoiseParamete
 from coach_b200.filters.filter import InputFilter, ObservationNormalizationFilter
 from coach_b200.memories.episodic_experience_replay import EpisodicExperienceReplayParameters
 from coach_b200.schedules import ConstantSchedule
-from coach_b200.utils import dynamic_import_and_instantiate_module_from_params, graph_capture
+from coach_b200.utils import dynamic_import_and_instantiate_module_from_params
 
 # discrete actions: the categorical softmax and draw of cb200_policy_act (acting and the old policy) take 1 .. 18 actions,
 # Atari's full action set; cb200_ppo_categorical_head itself takes up to 32
@@ -169,36 +172,27 @@ class ClippedPPOAgent(object):
         gen = torch.Generator().manual_seed(int(seed)) if seed is not None else None
         self.net.init(gen)
         st = self.net.store
-        self.theta_target = st.new_buffer()
+        self.main = _Net(self.lib, st, net_p, self.device)
         # the captured minibatch step holds its workspace's pointer; rollout-sized and acting passes, which may grow
         # theirs, use another
         self.ws, self.ws_rollout = Workspace(self.device), Workspace(self.device)
         dev, B = self.device, self.B
         f32 = lambda *s: torch.zeros(s, dtype=torch.float32, device=dev)     # noqa: E731
-        # persistent minibatch buffers
-        if self.discrete:
-            self.mb = dict(states=f32(B, self.D), actions=torch.zeros(B, dtype=torch.int64, device=dev),
-                           advantages=f32(B), value_targets=f32(B, 1), old_probs=f32(B, self.A))
-        else:
-            self.mb = dict(states=f32(B, self.D), actions=f32(B, self.A), advantages=f32(B), value_targets=f32(B, 1),
-                           old_mu=f32(B, self.A))
+        self.mb = self._columns(B)             # the minibatch the step gathers
         self.v_inst = self.net.v_seq.instantiate(self.lib, self.ws, B, self.mb["states"], st.theta, st.grad,
                                                  train=True)
         self.p_inst = self.net.p_seq.instantiate(self.lib, self.ws, B, self.mb["states"], st.theta, st.grad,
                                                  train=True)
         self.scalars = f32(5)
         self.v_loss = f32(1)
-        self.sumsq = f32(1)
-        self.adam_state = torch.tensor([net_p.adam_optimizer_beta1, net_p.adam_optimizer_beta2], dtype=torch.float32,
-                                       device=dev)
+        self.v_acc, self.p_acc = f32(1), f32(1)       # one epoch's sums of the value loss and the policy loss
         self.cursor = torch.zeros(1, dtype=torch.int64, device=dev)
         # the clipping schedule's value as the discrete head reads it (fp32, written at the start of every phase)
         self.clip_rescaler = f32(1)
-        self._graph = None
-        self._graph_key = None
+        self.clip_eps = None       # the head's fp32 clip epsilon launch argument, held by the step's graph
         self.graph_captures = 0
-        self._rows = None          # discrete: persistent rollout-sized training columns (capacity, dict, argmax scratch)
-        self._perm = None          # discrete: persistent permutation of the rollout rows
+        self._step = None          # the minibatch step (GraphedKernels)
+        self._rows = None          # persistent training columns (capacity, dict, permutation, argmax scratch)
         self._full = {}            # rollout-sized forward instances, keyed by N
         self._act = {}             # acting buffers, keyed by the number of environments
         self.training_iteration = 0
@@ -213,8 +207,7 @@ class ClippedPPOAgent(object):
 
     def sync(self):
         """online -> target: the frozen "old policy" (network_wrapper.py:94-107, clipped_ppo_agent.py:326)"""
-        _lib.check(self.lib.cb200_polyak(self.theta_target.data_ptr(), self.net.store.theta.data_ptr(),
-                                         self.net.store.size, 1.0, _lib.current_stream()))
+        self.main.sync()
 
     # ---- rollout-sized forward passes ------------------------------------------------------------------------------
     def _full_instances(self, N):
@@ -222,7 +215,7 @@ class ClippedPPOAgent(object):
             st = self.net.store
             x = torch.zeros((N, self.D), dtype=torch.float32, device=self.device)
             v = self.net.v_seq.instantiate(self.lib, self.ws_rollout, N, x, st.theta)
-            p_old = self.net.p_seq.instantiate(self.lib, self.ws_rollout, N, x, self.theta_target)
+            p_old = self.net.p_seq.instantiate(self.lib, self.ws_rollout, N, x, self.main.target)
             self._full = {N: (x, v, p_old)}           # keep only the latest size
         return self._full[N]
 
@@ -235,135 +228,98 @@ class ClippedPPOAgent(object):
         return rl_math.fill_advantages(rewards, values, game_overs, self.ap.algorithm.discount,
                                        self.ap.algorithm.gae_lambda)
 
-    # ---- one minibatch ---------------------------------------------------------------------------------------------
-    def _minibatch_kernels(self, data, perm, n_rows):
-        """all launches of one minibatch step; parameters independent of the minibatch index"""
+    # ---- training columns and one minibatch ----------------------------------------------------------------------
+    def _columns(self, n):
+        """n rows of what the minibatch step trains on: the actions (int64 [n] discrete, fp32 [n, A] continuous) and
+        the old policy (the target network's probabilities or means, [n, A])"""
+        f32 = lambda *s: torch.zeros(s, dtype=torch.float32, device=self.device)      # noqa: E731
+        actions = torch.zeros(n, dtype=torch.int64, device=self.device) if self.discrete else f32(n, self.A)
+        return dict(states=f32(n, self.D), actions=actions, advantages=f32(n), value_targets=f32(n, 1),
+                    old_policy=f32(n, self.A))
+
+    def _training_rows(self, n_rows):
+        """the persistent training columns, the permutation of their rows and the argmax scratch of the old policy's
+        softmax; grown when a phase trains on more rows, which rebuilds the minibatch step (its graph holds their
+        pointers)"""
+        if self._rows is None or self._rows[0] < n_rows:
+            i64 = lambda: torch.zeros(n_rows, dtype=torch.int64, device=self.device)      # noqa: E731
+            self._rows = (n_rows, self._columns(n_rows), i64(), i64())
+            self._step = None
+        return self._rows[1:]
+
+    def _minibatch_kernels(self):
+        """all launches of one minibatch step on the rows perm[cursor, cursor + B) of the training columns; parameters
+        independent of the minibatch index"""
         lib, st = self.lib, _lib.current_stream()
-        store = self.net.store
+        store, mb = self.main.store, self.mb
         alg, net_p = self.ap.algorithm, self.ap.network_wrappers["main"]
-        arr, cnt = _lib.make_columns([(data[k].data_ptr(), self.mb[k].data_ptr(),
-                                       self.mb[k].element_size() * int(np.prod(self.mb[k].shape[1:])))
-                                      for k in ("states", "actions", "advantages", "value_targets",
-                                                "old_probs" if self.discrete else "old_mu")])
+        _, cols, perm, _ = self._rows
+        arr, cnt = _lib.make_columns([(cols[k].data_ptr(), t.data_ptr(), t.element_size() * int(np.prod(t.shape[1:])))
+                                      for k, t in mb.items()])
         _lib.check(lib.cb200_gather_at(arr, cnt, perm.data_ptr(), self.cursor.data_ptr(), self.B, st))
         v = self.v_inst.forward()
         mu = self.p_inst.forward()
         # VHead: MSE(v, gae_based_value_target), loss weight 1 (v_head.py:41-44, head.py:172-177)
-        _lib.check(lib.cb200_regression_head_loss_grad(v.data_ptr(), self.mb["value_targets"].data_ptr(), None,
+        _lib.check(lib.cb200_regression_head_loss_grad(v.data_ptr(), mb["value_targets"].data_ptr(), None,
                                                        self.B, 1, 0, 1.0, self.v_inst.d_out.data_ptr(),
                                                        self.v_loss.data_ptr(), st))
         if self.discrete:
-            _lib.check(lib.cb200_ppo_categorical_head(mu.data_ptr(), self.mb["actions"].data_ptr(),
-                                                      self.mb["old_probs"].data_ptr(), self.mb["advantages"].data_ptr(),
-                                                      self.B, self.A, float(alg.clip_likelihood_ratio_using_epsilon),
+            _lib.check(lib.cb200_ppo_categorical_head(mu.data_ptr(), mb["actions"].data_ptr(),
+                                                      mb["old_policy"].data_ptr(), mb["advantages"].data_ptr(),
+                                                      self.B, self.A, float(self.clip_eps),
                                                       self.clip_rescaler.data_ptr(), float(alg.beta_entropy),
                                                       self.p_inst.d_out.data_ptr(), self.scalars.data_ptr(), st))
         else:
-            clip_eps = float(alg.clip_likelihood_ratio_using_epsilon) * float(alg.clipping_decay_schedule.current_value)
             logstd = store.view(store.theta, self.net.logstd_name)
-            old_logstd = store.view(self.theta_target, self.net.logstd_name)
+            old_logstd = store.view(self.main.target, self.net.logstd_name)
             d_logstd = store.view(store.grad, self.net.logstd_name)
-            _lib.check(lib.cb200_ppo_continuous_head(mu.data_ptr(), logstd.data_ptr(), self.mb["actions"].data_ptr(),
-                                                     self.mb["old_mu"].data_ptr(), old_logstd.data_ptr(),
-                                                     self.mb["advantages"].data_ptr(), self.B, self.A, clip_eps,
-                                                     float(alg.beta_entropy), self.p_inst.d_out.data_ptr(),
-                                                     d_logstd.data_ptr(), self.scalars.data_ptr(), st))
+            _lib.check(lib.cb200_ppo_continuous_head(mu.data_ptr(), logstd.data_ptr(), mb["actions"].data_ptr(),
+                                                     mb["old_policy"].data_ptr(), old_logstd.data_ptr(),
+                                                     mb["advantages"].data_ptr(), self.B, self.A,
+                                                     float(self.clip_eps), float(alg.beta_entropy),
+                                                     self.p_inst.d_out.data_ptr(), d_logstd.data_ptr(),
+                                                     self.scalars.data_ptr(), st))
         self.v_inst.backward()
         self.p_inst.backward()
-        n = store.size
-        _lib.check(lib.cb200_sumsq(store.grad.data_ptr(), n, self.sumsq.data_ptr(), self.ws.ptr(), st))
-        if net_p.clip_gradients:
-            _lib.check(lib.cb200_clip_by_global_norm(store.grad.data_ptr(), n, self.sumsq.data_ptr(),
-                                                     float(net_p.clip_gradients), st))
-        scaler = parallel.allreduce_gradients(store.grad,
-                                              net_p.scale_down_gradients_by_number_of_workers_for_sync_training)
-        if scaler != 1.0:
-            _lib.check(lib.cb200_scale(store.grad.data_ptr(), n, float(scaler), st))
-        _lib.check(lib.cb200_adam_tf_dev(store.theta.data_ptr(), store.m.data_ptr(), store.v.data_ptr(),
-                                         store.grad.data_ptr(), n, float(net_p.learning_rate),
-                                         float(net_p.adam_optimizer_beta1), float(net_p.adam_optimizer_beta2),
-                                         float(net_p.optimizer_epsilon), self.adam_state.data_ptr(), st))
+        self.main.apply(self.ws, ("ClipByGlobalNorm", net_p.clip_gradients) if net_p.clip_gradients else None)
+        _lib.check(lib.cb200_axpby_2d(self.v_loss.data_ptr(), 1, 1, 1, 1.0, 1.0, self.v_acc.data_ptr(), 1, st))
+        _lib.check(lib.cb200_axpby_2d(self.scalars.data_ptr(), 1, 1, 1, 1.0, 1.0, self.p_acc.data_ptr(), 1, st))
         _lib.check(lib.cb200_add_i64(self.cursor.data_ptr(), self.B, st))
+        self.graph_captures += torch.cuda.is_current_stream_capturing()      # the step's graph is capturing this call
 
-    def train_network(self, data, n_rows, epochs):
-        """clipped_ppo_agent.py:209-308.  data: dict of rollout-sized CUDA tensors (states, actions, advantages,
-        value_targets, and old_mu, or old_probs for discrete actions: int64 actions [N] and the old policy's
-        probabilities [N, A]).  Returns the mean [value loss, policy loss] of the last epoch as device tensors."""
-        B = self.B
+    def train_network(self, n_rows, epochs):
+        """clipped_ppo_agent.py:209-308 on the first n_rows rows of the training columns.  Returns the mean [value loss,
+        policy loss] of the last epoch as device tensors."""
+        alg, B = self.ap.algorithm, self.B
         n_full = n_rows // B
         if n_rows % B:
             raise ValueError("the rollout length (%d) must be a multiple of the batch size (%d)" % (n_rows, B))
+        # the clipping schedule's value: the discrete head reads it from the device rescaler, the continuous head takes
+        # fp32(epsilon * value) as its launch argument.  The step's graph holds that argument, so a new value rebuilds
+        # the step.
+        value = float(alg.clipping_decay_schedule.current_value)
+        self.clip_rescaler.fill_(value)
+        clip_eps = np.float32(float(alg.clip_likelihood_ratio_using_epsilon) * (1.0 if self.discrete else value))
+        if self._step is None or clip_eps != self.clip_eps:
+            self.clip_eps = clip_eps
+            self._step = GraphedKernels(self._minibatch_kernels, self.device)
+            # several ranks run the step eagerly, their all-reduces outside any graph
+            self._step.enabled &= self.use_cuda_graph and self.device.type == "cuda" and parallel.world()[1] == 1
+        perm = self._rows[2]
         # one pinned row per epoch: an epoch's asynchronous copy may still be queued when the host shuffles the next
         perm_host = torch.zeros((epochs, n_rows), dtype=torch.int64, pin_memory=self.device.type == "cuda")
-        if self.discrete:
-            # the clipping schedule reaches the head through the device rescaler, so the key leaves it out and one
-            # graph serves every phase that trains on the same columns
-            if self._perm is None or self._perm.numel() < n_rows:
-                self._perm = torch.zeros(n_rows, dtype=torch.int64, device=self.device)
-            perm = self._perm
-            key = (tuple(t.data_ptr() for t in data.values()), perm.data_ptr())
-            self.clip_rescaler.fill_(float(self.ap.algorithm.clipping_decay_schedule.current_value))
-        else:
-            perm = torch.zeros(n_rows, dtype=torch.int64, device=self.device)
-            key = (tuple(t.data_ptr() for t in data.values()), perm.data_ptr(), n_rows,
-                   float(self.ap.algorithm.clipping_decay_schedule.current_value))
-        world = parallel.world()[1]
-        graphable = self.use_cuda_graph and self.device.type == "cuda" and world == 1
-        if graphable and self.discrete and key == self._graph_key:
-            graph = self._graph
-        elif graphable:
-            # warm-up launch outside capture (lazy module loading), then capture once.  The warm-up gathers at the
-            # cursor, which a previous phase left at its rollout's end: start it at row 0, inside this permutation.
-            self.cursor.zero_()
-            side = torch.cuda.Stream()
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                self._snapshot_then_restore(lambda: self._minibatch_kernels(data, perm, n_rows))
-            torch.cuda.current_stream().wait_stream(side)
-            graph = torch.cuda.CUDAGraph()
-            with graph_capture(graph):
-                self._minibatch_kernels(data, perm, n_rows)
-            self._restore_snapshot()
-            self._graph, self._graph_key = graph, key
-            self.graph_captures += 1
         order = list(range(n_rows))
-        v_acc = torch.zeros(1, dtype=torch.float32, device=self.device)
-        p_acc = torch.zeros(1, dtype=torch.float32, device=self.device)
         for epoch in range(epochs):
             random.shuffle(order)                                   # batch.shuffle(), core_types.py:452-468
             perm_host[epoch].copy_(torch.tensor(order, dtype=torch.int64))
             perm[:n_rows].copy_(perm_host[epoch], non_blocking=True)
             self.cursor.zero_()
-            v_acc.zero_()
-            p_acc.zero_()
-            for i in range(n_full):
-                if graphable:
-                    graph.replay()
-                else:
-                    self._minibatch_kernels(data, perm, n_rows)
-                v_acc += self.v_loss
-                p_acc += self.scalars[0:1]
-        self.last_losses = (v_acc / n_full, p_acc / n_full)
+            self.v_acc.zero_()
+            self.p_acc.zero_()
+            for _ in range(n_full):
+                self._step()
+        self.last_losses = (self.v_acc / n_full, self.p_acc / n_full)
         return self.last_losses
-
-    # snapshot / restore of everything a warm-up or capture pass mutates (weights, Adam slots + state, cursor)
-    def _snapshot_then_restore(self, fn):
-        self._take_snapshot()
-        fn()
-        self._restore_snapshot()
-
-    def _take_snapshot(self):
-        s = self.net.store
-        self._snap = (s.theta.clone(), s.m.clone(), s.v.clone(), self.adam_state.clone(), self.cursor.clone())
-
-    def _restore_snapshot(self):
-        s = self.net.store
-        th, m, v, ad, cur = self._snap
-        s.theta.copy_(th)
-        s.m.copy_(m)
-        s.v.copy_(v)
-        self.adam_state.copy_(ad)
-        self.cursor.copy_(cur)
 
     # ---- driver ----------------------------------------------------------------------------------------------------
     def _should_train(self):
@@ -383,13 +339,8 @@ class ClippedPPOAgent(object):
         if self.pre_network_filter is not None:
             batch = self.pre_network_filter.filter(batch, deep_copy=False,
                                                    update_internal_state=alg.update_pre_network_filters_state_on_train)
-        states = batch.states(["observation"])["observation"].to(torch.float32).contiguous()
-        if self.discrete:
-            self._train_discrete(batch, states)
-            self.memory.clean()
-            self.training_iteration += 1
-            return None
-        actions = batch.actions().to(torch.float32).reshape(batch.size, self.A).contiguous()
+        states = batch.states(["observation"])["observation"].to(torch.float32)
+        actions = batch.actions().reshape((batch.size,) + self.mb["actions"].shape[1:])
         for _ in range(alg.num_consecutive_training_steps):
             self.sync()
             adv, tgt, n_valid = self.fill_advantages(states, batch.rewards(), batch.game_overs())
@@ -402,52 +353,24 @@ class ClippedPPOAgent(object):
             # whole minibatches only: the reference also trains on the partial tail batch (clipped_ppo_agent.py:225,
             # ceil(size / batch_size)); with the presets' 2048-step rollouts and batch 64 there is none
             n_rows = (n_rows // self.B) * self.B
+            cols, _, argmax = self._training_rows(n_rows)
             _, _, p_old = self._full_instances(batch.size)
-            old_mu = p_old.forward()                                   # frozen target network, whole rollout at once
-            f32 = lambda t: t.to(torch.float32).contiguous()           # noqa: E731
-            data = dict(states=states, actions=actions, advantages=f32(adv), value_targets=f32(tgt).reshape(-1, 1),
-                        old_mu=old_mu)
-            self.train_network(data, n_rows, alg.optimization_epochs)
-        self.memory.clean()                                            # post_training_commands :310-312
-        self.training_iteration += 1
-        return None
-
-    def _training_rows(self, n_rows):
-        """discrete: the persistent training columns and the scratch argmax of the old-policy softmax, grown when a
-        phase trains on more rows (the captured graph holds their pointers)"""
-        if self._rows is None or self._rows[0] < n_rows:
-            f32 = lambda *s: torch.zeros(s, dtype=torch.float32, device=self.device)      # noqa: E731
-            cols = dict(states=f32(n_rows, self.D), actions=torch.zeros(n_rows, dtype=torch.int64, device=self.device),
-                        advantages=f32(n_rows), value_targets=f32(n_rows, 1), old_probs=f32(n_rows, self.A))
-            self._rows = (n_rows, cols, torch.zeros(n_rows, dtype=torch.int64, device=self.device))
-        return self._rows[1], self._rows[2]
-
-    def _train_discrete(self, batch, states):
-        """the discrete branch of train(): actions stay int64, the old policy is the target network's softmax"""
-        alg = self.ap.algorithm
-        actions = batch.actions().reshape(batch.size).to(torch.int64)
-        for _ in range(alg.num_consecutive_training_steps):
-            self.sync()
-            adv, tgt, n_valid = self.fill_advantages(states, batch.rewards(), batch.game_overs())
-            n_rows = batch.size
-            if alg.truncate_dataset_to_playing_steps:
-                n_rows = min(n_rows, alg.num_consecutive_playing_steps.num_steps)
-            if n_rows < self.B:
-                raise ValueError("the rollout holds %d transitions, fewer than one minibatch of %d: nothing to train on "
-                                 "(the reference would train on one partial minibatch)" % (n_rows, self.B))
-            n_rows = (n_rows // self.B) * self.B
-            cols, argmax = self._training_rows(n_rows)
-            _, _, p_old = self._full_instances(batch.size)
-            logits_old = p_old.forward()                               # frozen target network, whole rollout at once
-            # the old policy's probabilities: the categorical softmax of the acting code (its argmax is not used)
-            _lib.check(self.lib.cb200_policy_act(logits_old.data_ptr(), n_rows, self.A, 0, None, None, None,
-                                                 argmax.data_ptr(), cols["old_probs"].data_ptr(), None, None,
-                                                 _lib.current_stream()))
+            old = p_old.forward()                                      # frozen target network, whole rollout at once
+            if self.discrete:
+                # the old policy's probabilities: the categorical softmax of the acting code (its argmax is not used)
+                _lib.check(self.lib.cb200_policy_act(old.data_ptr(), n_rows, self.A, 0, None, None, None,
+                                                     argmax.data_ptr(), cols["old_policy"].data_ptr(), None, None,
+                                                     _lib.current_stream()))
+            else:
+                cols["old_policy"][:n_rows].copy_(old[:n_rows])
             cols["states"][:n_rows].copy_(states[:n_rows])
             cols["actions"][:n_rows].copy_(actions[:n_rows])
             cols["advantages"][:n_rows].copy_(adv[:n_rows])
             cols["value_targets"][:n_rows].copy_(tgt[:n_rows].reshape(-1, 1))
-            self.train_network(cols, n_rows, alg.optimization_epochs)
+            self.train_network(n_rows, alg.optimization_epochs)
+        self.memory.clean()                                            # post_training_commands :310-312
+        self.training_iteration += 1
+        return None
 
     # ---- acting ------------------------------------------------------------------------------------------------------
     def _act_buffers(self, E):
@@ -517,8 +440,8 @@ class ClippedPPOAgent(object):
 
     # ---- checkpoint host state ---------------------------------------------------------------------------------------
     def checkpoint_state(self):
-        """the clipping schedule's value, and the noise schedule's for continuous actions (the networks go through the
-        ClippedPPO checkpoint item)"""
+        """the clipping schedule's value, and the noise schedule's for continuous actions (the network goes through the
+        ``main`` checkpoint item)"""
         state = dict(clipping=float(self.ap.algorithm.clipping_decay_schedule.current_value))
         if not self.discrete:
             state["noise"] = float(self.noise_schedule.current_value)

@@ -182,8 +182,6 @@ def _network_items(agent):
         net = getattr(agent, tag, None)
         if net is not None and hasattr(net, "store") and hasattr(net, "adam_state"):
             out.append((tag, net.store, {"adam_state": net.adam_state, "target": net.target}, net))
-    if hasattr(agent, "net") and hasattr(agent.net, "store") and hasattr(agent, "theta_target"):   # ClippedPPO
-        out.append(("main", agent.net.store, {"adam_state": agent.adam_state, "target": agent.theta_target}, agent))
     return out
 
 

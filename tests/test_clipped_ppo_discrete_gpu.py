@@ -3,10 +3,11 @@
   cb200_ppo_categorical_head at the C ABI: A in {1, 2, 3, 18, 32} x B in {1, 64, 1000, 4096} x beta in {0, 0.01} within
   fp64 bounds, every clipping regime, an exact probe (old = new), out-of-range actions, argument errors, one launch per
   call, bit-identical repeats and a captured graph that follows the device rescaler;
-  the agent: one minibatch step, whole training phases (eager and graph), one graph capture across phases while the
-  clipping schedule moves, acting for both action kinds, and a checkpoint round trip.
+  the agent: one minibatch step, whole training phases (eager and graph), the graph captures across phases while the
+  clipping schedule moves or stays put, acting and a checkpoint round trip for both action kinds.
 
 Generated ratios keep a margin from the clip bounds 1 -+ e, where fp32 and fp64 could pick different branches."""
+import os
 import random
 
 import numpy as np
@@ -223,16 +224,23 @@ def _params(schedule=None, beta=0.01, epochs=2, playing=256, B=64):
     return ap
 
 
-def _agent(A=3, D=8, graph=True, seed=0, **kw):
+def _agent(A=3, D=8, graph=True, seed=0, continuous=False, **kw):
+    """discrete actions, or continuous ones bounded to [-2, 2]"""
     from coach_b200.agents.clipped_ppo_agent import ClippedPPOAgent
-    ag = ClippedPPOAgent(_params(**kw), observation_dim=D, num_actions=A, seed=seed)
+    space = dict(action_dim=A, action_low=-2.0, action_high=2.0) if continuous else dict(num_actions=A)
+    ag = ClippedPPOAgent(_params(**kw), observation_dim=D, seed=seed, **space)
     ag.use_cuda_graph = graph
     return ag
 
 
-def _rollout(rng, n, D, A, ep_len):
+def _draws(rng, E, A, continuous=False):
+    """choose_actions' training draws for E environments"""
+    return dict(normals=rng.standard_normal((E, A))) if continuous else dict(uniforms=rng.random_sample(E))
+
+
+def _rollout(rng, n, D, A, ep_len, continuous=False):
     s = (rng.randn(n, D) * 2 + 0.3).astype(np.float32)
-    a = rng.randint(0, A, n).astype(np.int64)
+    a = rng.randn(n, A).astype(np.float32) if continuous else rng.randint(0, A, n).astype(np.int64)
     r = rng.randn(n)
     done = np.zeros(n, np.uint8)
     done[ep_len - 1::ep_len] = 1
@@ -269,7 +277,7 @@ def test_minibatch_step_matches_oracle(beta):
     ag.sync()
     store.theta.add_(torch.from_numpy(rng.randn(store.size).astype(np.float32) * 0.2).cuda())
     named = store.export_named()
-    old_named = store.export_named(ag.theta_target)
+    old_named = store.export_named(ag.main.target)
     states = rng.randn(B, D).astype(np.float32)
     q = oc.old_probs(old_named, states)
     logits = oac.mlp([torch.from_numpy(v).double() for v in list(named.values())[7:13]], torch.from_numpy(states)
@@ -292,17 +300,22 @@ def test_minibatch_step_matches_oracle(beta):
     data = dict(states=torch.from_numpy(states).to(dev), actions=torch.from_numpy(acts).to(dev),
                 advantages=torch.from_numpy(mb["advantages"]).to(dev),
                 value_targets=torch.from_numpy(mb["value_targets"]).reshape(-1, 1).to(dev),
-                old_probs=torch.from_numpy(q).to(dev))
-    perm = torch.arange(B, dtype=torch.int64, device=dev)
+                old_policy=torch.from_numpy(q).to(dev))
+    cols, perm, _ = ag._training_rows(B)
+    for k, t in data.items():
+        cols[k].copy_(t)
+    perm.copy_(torch.arange(B, dtype=torch.int64, device=dev))
     ag.cursor.zero_()
+    ag.clip_eps = np.float32(EPS)
     ag.clip_rescaler.fill_(0.8)
-    ag._minibatch_kernels(data, perm, B)
+    ag._minibatch_kernels()
     torch.cuda.synchronize()
     close(ag.v_loss.item(), ref["value_loss"], name="value loss")
     sc = ag.scalars.cpu().numpy()
     for k, name in enumerate(("policy loss", "kl", "entropy", "mean ratio", "mean clipped ratio")):
         close(sc[k], ref["scalars"][k], atol=1e-6, name=name)
-    close(np.sqrt(ag.sumsq.item()), ref["grad_norm"], name="grad norm")
+    close(np.sqrt(ag.main.sumsq.item()), ref["grad_norm"], name="grad norm")
+    assert ag.v_acc.item() == ag.v_loss.item() and ag.p_acc.item() == sc[0]       # the epoch sums
     got = store.export_named(store.grad)
     for name in ref["grads"]:
         close(got[name], ref["grads"][name].numpy(), rtol=1e-4, name="grad " + name)
@@ -364,32 +377,50 @@ def test_training_phase_eager_and_graph_agree_and_match_the_oracle():
     assert agents[0].memory.num_transitions() == 0        # post_training_commands: memory.clean()
 
 
-def test_one_graph_across_phases_while_the_schedule_moves():
-    """the clipping schedule moves with acting between phases; the discrete graph is captured once and every phase
-    stays bit-identical to eager execution, so the replayed graph reads each phase's rescaler"""
-    from coach_b200.schedules import LinearSchedule
+def _phases_across_the_schedule(continuous, moving):
+    """three phases with acting between them, eager and graph: every phase stays bit-identical to eager execution.
+    The discrete graph is captured once, so the replayed graph reads each phase's rescaler; the continuous step takes
+    fp32(epsilon * value) as a launch argument and is captured once per distinct value."""
+    from coach_b200.schedules import ConstantSchedule, LinearSchedule
     # ten epochs, as the presets train: each epoch's permutation must reach the device intact while the host shuffles
     # the next one
-    agents = [_agent(graph=g, schedule=LinearSchedule(1.0, 0.0, 600), epochs=10) for g in (False, True)]
+    agents = [_agent(graph=g, continuous=continuous, epochs=10,
+                     schedule=LinearSchedule(1.0, 0.0, 600) if moving else ConstantSchedule(0.7)) for g in (False, True)]
     rng = np.random.RandomState(3)
     values = []
     for phase in range(3):
-        roll = _rollout(rng, 256, 8, 3, 40)
+        roll = _rollout(rng, 256, 8, 3, 40, continuous)
         states = rng.randn(64, 8).astype(np.float32)
-        u = rng.random_sample(64)
+        draws = _draws(rng, 64, 3, continuous)
         for ag in agents:
-            ag.choose_actions(states, uniforms=u)
+            ag.choose_actions(states, **draws)
             _store(ag, roll)
             random.seed(10 + phase)
             ag.train()
         values.append(agents[1].ap.algorithm.clipping_decay_schedule.current_value)
         torch.cuda.synchronize()
-        assert float(agents[1].clip_rescaler.item()) == np.float32(values[-1])
+        if not continuous:
+            assert float(agents[1].clip_rescaler.item()) == np.float32(values[-1])
         a, b = agents[0].net.store.export_named(), agents[1].net.store.export_named()
         for name in a:
             assert_bits(b[name], a[name], "phase %d %s" % (phase, name))
-    assert len(set(values)) == 3
-    assert agents[1].graph_captures == 1
+        for x, y, name in zip(agents[0].last_losses, agents[1].last_losses, ("value loss", "policy loss")):
+            assert_bits(y.cpu().numpy(), x.cpu().numpy(), "phase %d %s" % (phase, name))
+    assert len(set(values)) == (3 if moving else 1)
+    eps = {np.float32(agents[1].ap.algorithm.clip_likelihood_ratio_using_epsilon * v) for v in values}
+    assert agents[1].graph_captures == (len(eps) if continuous else 1) and agents[0].graph_captures == 0
+
+
+def test_one_graph_across_phases_while_the_schedule_moves():
+    """the clipping schedule moves with acting between phases; the discrete graph is captured once"""
+    _phases_across_the_schedule(continuous=False, moving=True)
+
+
+@pytest.mark.parametrize("moving", [False, True], ids=["constant", "moving"])
+def test_continuous_graph_captures_follow_the_clip_epsilon(moving):
+    """a schedule that stays put between phases captures the continuous step once; a moving one once per distinct
+    fp32 epsilon"""
+    _phases_across_the_schedule(continuous=True, moving=moving)
 
 
 def _oracle_probs(ag, states):
@@ -452,17 +483,21 @@ def test_continuous_acting_draws_numpy_normal_and_steps_both_schedules():
     assert ag.noise_schedule.current_value == oc.schedule_values(LinearSchedule(0.5, 0.1, 50), E)[-1]
 
 
-def test_checkpoint_restore_then_next_phase_is_bit_identical(tmp_path):
+def _checkpoint_round_trip(tmp_path, continuous):
+    """save after a phase and acting, restore into an agent built from another seed, train one more phase in both"""
     from coach_b200 import checkpoint
     from coach_b200.schedules import LinearSchedule
     rng = np.random.RandomState(7)
-    rolls = [_rollout(rng, 256, 8, 3, 64) for _ in range(2)]
-    a = _agent(schedule=LinearSchedule(1.0, 0.0, 500), seed=0)
+    rolls = [_rollout(rng, 256, 8, 3, 64, continuous) for _ in range(2)]
+    a = _agent(schedule=LinearSchedule(1.0, 0.0, 500), seed=0, continuous=continuous)
     _store(a, rolls[0])
     a.train()
-    a.choose_actions(rng.randn(32, 8).astype(np.float32), uniforms=rng.random_sample(32))
+    a.choose_actions(rng.randn(32, 8).astype(np.float32), **_draws(rng, 32, 3, continuous))
     name = checkpoint.save_checkpoint(a, str(tmp_path))
-    b = _agent(schedule=LinearSchedule(1.0, 0.0, 500), seed=3)
+    # the network's files: weights, Adam slots, Adam state and the target buffer
+    assert sorted(f[len(name) + 1:] for f in os.listdir(str(tmp_path)) if f.startswith(name + ".net_")) == \
+        sorted("net_main.%s.npy" % k for k in ("theta", "m", "v", "adam_state", "target"))
+    b = _agent(schedule=LinearSchedule(1.0, 0.0, 500), seed=3, continuous=continuous)
     checkpoint.restore_checkpoint(b, str(tmp_path), name)
     assert b.ap.algorithm.clipping_decay_schedule.current_value == a.ap.algorithm.clipping_decay_schedule.current_value
     for ag in (a, b):
@@ -474,3 +509,13 @@ def test_checkpoint_restore_then_next_phase_is_bit_identical(tmp_path):
     for k in x:
         assert_bits(y[k], x[k], k)
     assert_bits(b.net.store.m.cpu().numpy(), a.net.store.m.cpu().numpy(), "adam m")
+    assert_bits(b.main.target.cpu().numpy(), a.main.target.cpu().numpy(), "target")
+    assert_bits(b.main.adam_state.cpu().numpy(), a.main.adam_state.cpu().numpy(), "adam state")
+
+
+def test_checkpoint_restore_then_next_phase_is_bit_identical(tmp_path):
+    _checkpoint_round_trip(tmp_path, continuous=False)
+
+
+def test_continuous_checkpoint_restore_then_next_phase_is_bit_identical(tmp_path):
+    _checkpoint_round_trip(tmp_path, continuous=True)

@@ -52,7 +52,7 @@ def test_ppo_head_and_minibatch_step_match_oracle(beta):
     store.theta.add_(torch.randn(store.size, device=store.theta.device, generator=None) * 0.02)
     store.view(store.theta, ag.net.logstd_name).copy_(torch.tensor(rng.randn(A).astype(np.float32) * 0.3))
     named = store.export_named()
-    old_named = store.export_named(ag.theta_target)
+    old_named = store.export_named(ag.main.target)
     mb = dict(states=rng.randn(B, D).astype(np.float32), actions=rng.randn(B, A).astype(np.float32),
               advantages=rng.randn(B).astype(np.float32), value_targets=rng.randn(B).astype(np.float32))
     opt = oac.make_adam(named, 3e-4, 0.9, 0.999, 1e-5)
@@ -63,16 +63,21 @@ def test_ppo_head_and_minibatch_step_match_oracle(beta):
     data = dict(states=torch.from_numpy(mb["states"]).to(dev), actions=torch.from_numpy(mb["actions"]).to(dev),
                 advantages=torch.from_numpy(mb["advantages"]).to(dev),
                 value_targets=torch.from_numpy(mb["value_targets"]).reshape(-1, 1).to(dev),
-                old_mu=torch.from_numpy(ref["old_mu"]).to(dev))
-    perm = torch.arange(B, dtype=torch.int64, device=dev)
+                old_policy=torch.from_numpy(ref["old_mu"]).to(dev))
+    cols, perm, _ = ag._training_rows(B)
+    for k, t in data.items():
+        cols[k].copy_(t)
+    perm.copy_(torch.arange(B, dtype=torch.int64, device=dev))
     ag.cursor.zero_()
-    ag._minibatch_kernels(data, perm, B)
+    ag.clip_eps = np.float32(0.2)
+    ag._minibatch_kernels()
     torch.cuda.synchronize()
     close(ag.v_loss.item(), ref["value_loss"], name="value loss")
     close(ag.scalars[0].item(), ref["policy_loss"], name="policy loss")
     close(ag.scalars[3].item(), ref["mean_ratio"], name="mean ratio")
     close(ag.scalars[2].item(), ref["entropy"], name="entropy")
-    close(np.sqrt(ag.sumsq.item()), ref["grad_norm"], name="grad norm")
+    close(np.sqrt(ag.main.sumsq.item()), ref["grad_norm"], name="grad norm")
+    assert ag.v_acc.item() == ag.v_loss.item() and ag.p_acc.item() == ag.scalars[0].item()   # the epoch sums
     got = store.export_named(store.grad)
     for name in ref["grads"]:
         close(got[name], ref["grads"][name].numpy(), name="grad " + name)
